@@ -1,13 +1,14 @@
 #!/usr/bin/env python
-"""bench.py -- the hot path of BASELINE.json on B200: brute-force IP top-10 over a 10M x 1024 bf16 index
+"""bench.py -- the hot path of BASELINE.json on H100: brute-force IP top-10 over a 10M x 1024 bf16 index
 (queries/sec) and BGE-large index-build encode (chunks/sec).
 
     python bench.py [--gpus N --steps K --warmup W]            # our arm, one JSON line on stdout
+    python bench.py --dump-outputs DIR [...]                   # also write the last timed step's results as DIR/*.npy
     python bench.py --impl reference [...]                     # the reference's CPU path, same metric
-    torchrun --nproc-per-node N bench.py --gpus N ...          # N > 1: one rank per GPU (launched by the driver)
+    torchrun --nproc-per-node N bench.py --gpus N ...          # N > 1: one rank per GPU
 
 A "step" is one pass of the search hot path over one batch of 32 synthetic probe queries (config 5's probe
-batch) against the whole index: N=1 holds all 10M rows on one GPU (20.5 GB bf16); at N>1 the SAME 10M rows are
+batch) against the whole index: N=1 holds all 10M rows on one 80 GB GPU (20.5 GB bf16); at N>1 the SAME 10M rows are
 row-sharded over the ranks ("strong" scaling: total work fixed).  A step is ONE CUDA-graph launch holding the shard
 scan kernel and the fused finalize kernel -- at N>1 the finalize kernel also pushes the rank's top-k record into
 every peer's buffer over NVLink and merges all ranks' records (crag_search_finalize_exchange), or, when symmetric
@@ -54,6 +55,9 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="launch the step's kernels one by one instead of one CUDA graph")
     ap.add_argument("--cpu-budget-s", type=float, default=20.0, help="CPU baseline sample budget (seconds of queries)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed search step returned (ids, scores, min/max) and the "
+                         "last timed encode step's embeddings as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -67,7 +71,7 @@ def workload_config(rows: int, dim: int, nq: int, k: int, world: int) -> dict:
     return {"workload": f"{rows}x{dim} bf16 index, brute-force IP top-{k}, {nq} probe queries per step, "
                         f"row-sharded over {world} GPU(s)",
             "index_rows": rows, "rows_per_rank": rows_rank0, "dim": dim, "queries_per_step": nq, "k": k,
-            "l2": f"inputs larger than L2 ({rows_rank0 * dim * 2 / 1e9:.2f} GB shard per rank vs 126 MB)"}
+            "l2": f"inputs larger than L2 ({rows_rank0 * dim * 2 / 1e9:.2f} GB shard per rank vs 50 MB)"}
 
 
 def load_peaks():
@@ -76,24 +80,13 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
-
-
-def scan_traffic(rows: int, dim: int, nq: int, k: int):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one scan launch from the committed `ncu --set full` capture
-    (profiles/search_traffic.json), if one exists for exactly this shard shape; else None."""
-    p = os.path.join(ROOT, "profiles", "search_traffic.json")
-    if not os.path.exists(p):
-        return None
-    for e in json.load(open(p)):
-        if (e["rows"], e["dim"], e["nq"], e["k"]) == (rows, dim, nq, k):
-            return e["dram_bytes"]
-    return None
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- upper bounds, not measured rates
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 # ------------------------------------------------------------------------------------------ clocks sampler
 class ClockSampler:
-    """nvidia-smi sampled every 100 ms while the timed region runs (B200_PROFILING.md recipe)."""
+    """nvidia-smi sampled every 100 ms while the timed region runs."""
 
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -143,9 +136,9 @@ class ClockSampler:
 
 # ------------------------------------------------------------------------------------------ the reference's modules
 def find_reference_root():
-    """The reference checkout in the build container, or the unmodified copy tools/stage_reference.sh puts under
-    baseline/_ref (git-ignored, travels to the GPU box)."""
-    for cand in (os.environ.get("COMORAG_REFERENCE"), "/root/reference", os.path.join(ROOT, "baseline", "_ref")):
+    """The reference checkout named by $COMORAG_REFERENCE, else the unmodified copy build() stages under oracle/_ref;
+    None when neither exists (the CPU arms then use the oracle port)."""
+    for cand in (os.environ.get("COMORAG_REFERENCE"), os.path.join(ROOT, "oracle", "_ref")):
         if cand and os.path.isdir(os.path.join(cand, "src", "comorag")):
             return cand
     return None
@@ -457,6 +450,16 @@ def count_id_mismatches(got_ids, want_ids, want_scores, k: int, tie: float = 2e-
     return int(bad)
 
 
+def dump_outputs(out_dir: str, ids, scores, minmax) -> None:
+    """What a caller of the timed path receives, as float64 / float32 .npy files (ids are < 2^53, exact in float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "ids.npy"), ids.cpu().numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "scores.npy"), scores.float().cpu().numpy())
+    if minmax is not None:
+        np.save(os.path.join(out_dir, "minmax.npy"), minmax.float().cpu().numpy())
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -534,6 +537,8 @@ def run_ours(args):
     value = args.nq / ms_per_step * 1e3
     got_ids = session.ids.clone()
     got_scores = session.scores.clone()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, got_ids, got_scores, getattr(session, "minmax", None))
     if index.peer is not None:
         index.peer.check()
 
@@ -660,7 +665,7 @@ def run_ours(args):
             "planted_neighbours": planted,
             "clocks": clocks,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                         "frac": achieved / peaks["hbm_gbs"], "traffic": scan_traffic(my_rows, args.dim, args.nq, args.k),
+                         "frac": achieved / peaks["hbm_gbs"], "traffic": None,
                          "peak_source": peaks["source"],
                          "kernel": "search_topk_kernel", "algorithmic_bytes_per_launch": algo_bytes,
                          "kernel_ms": scan_avg, "step_ms_same_loop": sum(step_ms) / len(step_ms)},
@@ -700,6 +705,9 @@ def bench_encode(args, world, rank, dev, st, peaks, barrier, max_over_ranks):
     b.record(st)
     barrier()
     enc_ms = max_over_ranks(a.elapsed_time(b)) / args.encode_steps
+    if args.dump_outputs and rank == 0:   # the pooled, normalised embeddings of the last timed encode step
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "encode_embeddings.npy"), out.float().cpu().numpy())
     chunks_s = world * n / enc_ms * 1e3
     flops = cfg.flops_per_chunk(L) * n
     enc_tflops = flops / enc_ms / 1e9

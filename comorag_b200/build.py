@@ -1,7 +1,7 @@
-"""Build recipe for libcomorag_b200.so (hand-written sm_100a CUDA, C ABI).
+"""Build recipe for libcomorag_b200.so (hand-written sm_90a CUDA, C ABI).
 
-nvcc cross-compiles for sm_100a without a GPU, so this runs in the CPU-only
-build container; the resulting .so is git-ignored but travels to the GPU box.
+nvcc cross-compiles for sm_90a without a GPU, so the library can be built on a
+machine without one; the resulting .so is git-ignored.
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ LIB_PATH = LIB_DIR / "libcomorag_b200.so"
 INCLUDE = PKG_DIR.parent / "include"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--shared", "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fvisibility=hidden",
@@ -54,7 +54,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if not force and not _stale():
         LAST_BUILD_MODE = "up-to-date (every csrc/*.cu, *.cuh and include/*.h is older than the .so)"
         return LIB_PATH
-    LAST_BUILD_MODE = "compiled with nvcc -gencode arch=compute_100a,code=sm_100a"
+    LAST_BUILD_MODE = "compiled with nvcc -gencode arch=compute_90a,code=sm_90a"
     LIB_DIR.mkdir(parents=True, exist_ok=True)
     objs = []
     obj_dir = LIB_DIR / "obj"
@@ -77,7 +77,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if failed:
         raise RuntimeError("nvcc failed; see output above")
     tmp = LIB_PATH.with_suffix(".so.tmp")
-    link = [_nvcc(), "--shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(tmp), *map(str, objs)]
+    link = [_nvcc(), "--shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(tmp), *map(str, objs)]
     subprocess.run(link, check=True)
     os.replace(tmp, LIB_PATH)
     return LIB_PATH
@@ -95,7 +95,7 @@ def build_examples(force: bool = False) -> Path:
     if not force and EXAMPLE_BIN.exists() and all(p.stat().st_mtime <= EXAMPLE_BIN.stat().st_mtime for p in deps):
         return EXAMPLE_BIN
     EXAMPLE_BIN.parent.mkdir(parents=True, exist_ok=True)
-    cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-O2", "-std=c++17", "-lineinfo", "-I", str(INCLUDE),
+    cmd = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-lineinfo", "-I", str(INCLUDE),
            str(src), "-o", str(EXAMPLE_BIN), "-L", str(LIB_DIR), "-lcomorag_b200",
            "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN/../../comorag_b200/lib"]
     subprocess.run(cmd, check=True)

@@ -1,17 +1,14 @@
-// K2 on tcgen05: varlen multi-head self-attention for head dim 64 (BERT/BGE base & large).
+// K2 on wgmma: varlen multi-head self-attention for head dim 64 (BERT/BGE base & large).
 //
 //   ctx = softmax(Q K^T / sqrt(dh)) V      per (sequence, head), keys restricted to the sequence
 //
-// One CTA per (sequence, head, 128-query tile), two CTAs co-resident per SM.  192 threads:
-//   warp 0   TMA: Q tile once, then K_j / V_j blocks of 64 keys through 2-stage rings (128-byte swizzle, straight
+// One CTA per (sequence, head, 128-query tile).  288 threads:
+//   warps 0-7  two warpgroups, 64 query rows each: S_j = Q K_j^T (wgmma m64n64k16, Q and K_j from smem) into fp32
+//            registers, online softmax in registers (a row lives in the 4 lanes of a quad), P_j converted in place
+//            to the bf16 A fragment of O += P_j V_j (wgmma m64n64k16 with A from registers; V consumed MN-major,
+//            i.e. as stored), final O / l -> bf16 -> ctx
+//   warp 8   TMA: Q tile once, then K_j / V_j blocks of 64 keys through 2-stage rings (128-byte swizzle, straight
 //            out of the packed [T, 3H] qkv activation)
-//   warp 1   tcgen05.mma: S_j = Q K_j^T (M=128, N=64, K=64) into one of two TMEM score buffers;
-//            O += P_j V_j (M=128, N=64, K=64; V consumed MN-major, i.e. as stored) into TMEM columns [128,192)
-//   warps 2-5  softmax: thread = query row (one TMEM lane): tcgen05.ld the 64 scores, online max/sum in registers
-//            with LAZY rescaling (O is only rescaled in TMEM when the row max grew by > 2^8), P_j written to one of
-//            two smem buffers in the UMMA K-major 128B-swizzle layout, final O / l -> bf16 -> ctx.
-// S_{j+1} is issued as soon as the softmax warps have pulled S_{j-1} out of TMEM, so the exp2 stream (the MUFU
-// pipe is this kernel's roofline: 128 x L exp2 per tile) never waits for a tensor-core round trip.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -23,27 +20,11 @@ namespace crag {
 constexpr int kAttBM = 128;   // queries per CTA
 constexpr int kAttBN = 64;    // keys per block
 constexpr int kAttDH = 64;
-constexpr int kAttThreads = 192;
-constexpr uint32_t kAttTmemCols = 256;        // S0 [0,64) | S1 [64,128) | O [128,192)
-constexpr int kAttTileBytes = 128 * 64 * 2;   // 16 KB: Q tile, one P buffer
+constexpr int kAttThreads = 288;
+constexpr int kAttTileBytes = 128 * 64 * 2;   // 16 KB: Q tile
 constexpr int kAttKVBytes = kAttBN * 64 * 2;  // 8 KB: one K or V block
-// smem: Q 16K | K 2x8K | V 2x8K | P 2x16K | barriers  (~81 KB: two CTAs per SM)
-constexpr size_t kAttSmemBytes = 1024 + kAttTileBytes + 4 * kAttKVBytes + 2 * kAttTileBytes + 256;
-// (A "split" variant -- 8 softmax warps, two threads per query row -- was measured in round 2: 83.5 us against 79.2 us
-// for this kernel on 32 x 512 tokens x 16 heads; removed.)
-
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// smem: Q 16K | K 2x8K | V 2x8K | barriers  (~49 KB: several CTAs per SM)
+constexpr size_t kAttSmemBytes = 1024 + kAttTileBytes + 4 * kAttKVBytes + 256;
 
 __device__ __forceinline__ float att_exp2(float x) {
   float y;
@@ -51,23 +32,12 @@ __device__ __forceinline__ float att_exp2(float x) {
   return y;
 }
 
-// Shared-memory descriptor for an MN-major operand stored as [K rows][64 MN elements = 128 B] with the 128-byte
-// swizzle (a TMA box of a row-major [keys, d] matrix): 8-row (K) groups are 1024 B apart (SBO); there is a single
-// 64-element MN block, so LBO is unused.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_f32_bmn(uint32_t M, uint32_t N) {
-  return umma_idesc_bf16_f32(M, N) | (1u << 16);  // b_major = MN
+__device__ __forceinline__ uint32_t att_pack_bf16x2(float a, float b) {
+  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&v);
 }
 
-__global__ void __launch_bounds__(kAttThreads, 2)
+__global__ void __launch_bounds__(kAttThreads, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_kv,
                     const int32_t* __restrict__ cu_seqlens, int H, float scale_log2e, __nv_bfloat16* __restrict__ ctx) {
   const int seq = blockIdx.z, head = blockIdx.y;
@@ -82,210 +52,135 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_const
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + kAttTileBytes;        // [2]
   uint8_t* sV = sK + 2 * kAttKVBytes;      // [2]
-  uint8_t* sP = sV + 2 * kAttKVBytes;      // [2] x 16 KB
-  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sP + 2 * kAttTileBytes);
+  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sV + 2 * kAttKVBytes);
   uint64_t* bar_k_full = bar_q + 1;        // [2]
-  uint64_t* bar_k_empty = bar_k_full + 2;  // [2]
-  uint64_t* bar_v_full = bar_k_empty + 2;  // [2]
-  uint64_t* bar_v_empty = bar_v_full + 2;  // [2]
-  uint64_t* bar_s_full = bar_v_empty + 2;  // [2] S_j landed in TMEM
-  uint64_t* bar_s_free = bar_s_full + 2;   // [2] S_j pulled into registers (4 warps)
-  uint64_t* bar_p_full = bar_s_free + 2;   // [2] P_j written (4 warps)
-  uint64_t* bar_p_free = bar_p_full + 2;   // [2] P_j V_j retired: buffer reusable
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_p_free + 2);
+  uint64_t* bar_v_full = bar_k_full + 2;   // [2]
+  uint64_t* bar_kv_empty = bar_v_full + 2; // [2] both warpgroups are done with K_j and V_j (8 warps)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_q);
-    tma_prefetch_desc(&tm_kv);
+  if (threadIdx.x == 0) {
     mbar_init(bar_q, 1);
     for (int s = 0; s < 2; ++s) {
       mbar_init(&bar_k_full[s], 1);
-      mbar_init(&bar_k_empty[s], 1);
       mbar_init(&bar_v_full[s], 1);
-      mbar_init(&bar_v_empty[s], 1);
-      mbar_init(&bar_s_full[s], 1);
-      mbar_init(&bar_s_free[s], 4);
-      mbar_init(&bar_p_full[s], 4);
-      mbar_init(&bar_p_free[s], 1);
+      mbar_init(&bar_kv_empty[s], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, kAttTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_o = tmem_base + 128;
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (warp == 8) {
+    if (lane == 0) {
+      tma_prefetch_desc(&tm_q);
+      tma_prefetch_desc(&tm_kv);
       mbar_arrive_expect_tx(bar_q, kAttTileBytes);
       tma_load_2d(&tm_q, bar_q, sQ, head * kAttDH, start + q0);
       for (int j = 0; j < n_blk; ++j) {
         const int st = j & 1;
         const uint32_t ph = (j >> 1) & 1;
-        mbar_wait(&bar_k_empty[st], ph ^ 1);
+        mbar_wait(&bar_kv_empty[st], ph ^ 1);
         mbar_arrive_expect_tx(&bar_k_full[st], kAttKVBytes);
         tma_load_2d(&tm_kv, &bar_k_full[st], sK + st * kAttKVBytes, H + head * kAttDH, start + j * kAttBN);
-        mbar_wait(&bar_v_empty[st], ph ^ 1);
         mbar_arrive_expect_tx(&bar_v_full[st], kAttKVBytes);
         tma_load_2d(&tm_kv, &bar_v_full[st], sV + st * kAttKVBytes, 2 * H + head * kAttDH, start + j * kAttBN);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16_f32(kAttBM, kAttBN);
-      constexpr uint32_t idesc_o = umma_idesc_bf16_f32_bmn(kAttBM, kAttDH);
-      const uint32_t q_addr = smem_u32(sQ);
-      auto issue_s = [&](int j) {
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        mbar_wait(&bar_k_full[st], ph);
-        mbar_wait(&bar_s_free[st], ph ^ 1);   // S_{j-2} has been pulled out of this buffer
-        tc_fence_after();
-        const uint32_t k_addr = smem_u32(sK + st * kAttKVBytes);
-#pragma unroll
-        for (int ks = 0; ks < kAttDH / 16; ++ks)
-          umma_f16(tmem_base + st * kAttBN, umma_desc_k_sw128(q_addr + ks * 32), umma_desc_k_sw128(k_addr + ks * 32),
-                   idesc_s, ks > 0);
-        umma_commit(&bar_k_empty[st]);
-        umma_commit(&bar_s_full[st]);
-      };
-      mbar_wait(bar_q, 0);
-      issue_s(0);
-      for (int j = 0; j < n_blk; ++j) {
-        if (j + 1 < n_blk) issue_s(j + 1);
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        mbar_wait(&bar_v_full[st], ph);
-        mbar_wait(&bar_p_full[st], ph);
-        tc_fence_after();
-        const uint32_t p_addr = smem_u32(sP + st * kAttTileBytes);
-        const uint32_t v_addr = smem_u32(sV + st * kAttKVBytes);
-#pragma unroll
-        for (int kk = 0; kk < kAttBN / 16; ++kk)
-          umma_f16(tmem_o, umma_desc_k_sw128(p_addr + kk * 32), umma_desc_mn_sw128(v_addr + kk * 16 * 128), idesc_o,
-                   (j > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(&bar_v_empty[st]);
-        umma_commit(&bar_p_free[st]);
-      }
-    }
-  } else {
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;  // query row within the tile == TMEM lane
-    const uint32_t lane_addr = uint32_t(quad * 32) << 16;
-    float m_run = -INFINITY, l_run = 0.f;
-    const int swz = r & 7;
-    for (int j = 0; j < n_blk; ++j) {
-      const int st = j & 1;
-      const uint32_t ph = (j >> 1) & 1;
-      mbar_wait(&bar_s_full[st], ph);
-      tc_fence_after();
-      uint32_t v[2][32];
-      tmem_ld_32x32b_x32(tmem_base + lane_addr + st * kAttBN, v[0]);
-      tmem_ld_32x32b_x32(tmem_base + lane_addr + st * kAttBN + 32, v[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_s_free[st]);   // the tensor core may overwrite this score buffer
-      const int kbase = j * kAttBN;
-      if (kbase + kAttBN > L) {  // only the last block of a sequence whose length is not a multiple of 64
-#pragma unroll
-        for (int c = 0; c < 2; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (kbase + c * 32 + i >= L) v[c][i] = 0xff800000u;  // -inf: exp2 -> 0, never the max
-      }
-      float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int c = 0; c < 2; ++c)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[c][i]));
-      const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3])) * scale_log2e;  // finite: >= 1 valid key
-      // Lazy rescaling: the reference point m_run only moves when the true max has grown by more than 2^8; until
-      // then p = exp2(s - m_run) may exceed 1 (<= 256), which fp32 sums and bf16 P hold without loss, and O / l is
-      // unchanged mathematically.  Saves the TMEM round trip of O for almost every block.
-      float alpha = 1.0f;
-      if (mx > m_run + 8.0f) {
-        alpha = att_exp2(m_run - mx);   // first block: exp2(-inf) = 0
-        m_run = mx;
-      }
-      if (j > 0 && __any_sync(0xffffffffu, alpha != 1.0f)) {
-        // P_{j-1} V_{j-1} retired (P_j V_j cannot start before this warp's p_full).  p_free[(j-1)&1] is at most one
-        // phase behind here (block j-1 already waited for P_{j-3} V_{j-3} on it), so the parity test is unambiguous.
-        mbar_wait(&bar_p_free[(j - 1) & 1], ((j - 1) >> 1) & 1);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < 2; ++c) {
-          uint32_t o[32];
-          tmem_ld_32x32b_x32(tmem_o + lane_addr + c * 32, o);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st_32x32b_x32(tmem_o + lane_addr + c * 32, o);
-        }
-        tmem_st_wait();
-      }
-      // p = exp2(s*scale - m) (masked keys: exp2(-inf) = 0), row sums in 4 chains, bf16 P into the swizzled tile
-      mbar_wait(&bar_p_free[st], ph ^ 1);   // P_{j-2} V_{j-2} no longer reads this buffer
-      uint8_t* p_row = sP + st * kAttTileBytes + r * 128;
-      float rs4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t packed[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float p0 = att_exp2(fmaf(__uint_as_float(v[c][2 * i]), scale_log2e, -m_run));
-          const float p1 = att_exp2(fmaf(__uint_as_float(v[c][2 * i + 1]), scale_log2e, -m_run));
-          rs4[i & 3] += p0 + p1;
-          __nv_bfloat162 b = __floats2bfloat162_rn(p0, p1);
-          packed[i] = *reinterpret_cast<uint32_t*>(&b);
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q)   // 32 keys = 4 x 16-byte chunks of the 128-byte row
-          *reinterpret_cast<uint4*>(p_row + (((c * 4 + q) ^ swz) * 16)) =
-              make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
-      }
-      l_run = l_run * alpha + ((rs4[0] + rs4[1]) + (rs4[2] + rs4[3]));
-      fence_proxy_async();   // P (generic-proxy stores) -> visible to the tensor core's async proxy
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_p_full[st]);
-    }
-    // epilogue: O / l -> bf16 -> ctx[start + q0 + r, head*64 .. +64)
-    mbar_wait(&bar_p_free[(n_blk - 1) & 1], ((n_blk - 1) >> 1) & 1);   // last P V retired (they retire in order)
-    tc_fence_after();
-    const float inv = 1.f / l_run;
-    const int row = q0 + r;
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      uint32_t o[32];
-      tmem_ld_32x32b_x32(tmem_o + lane_addr + c * 32, o);
-      tmem_ld_wait();
-      if (row < L) {
-        __nv_bfloat16* dst = ctx + int64_t(start + row) * H + head * kAttDH + c * 32;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint32_t w[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            __nv_bfloat162 b = __floats2bfloat162_rn(__uint_as_float(o[q * 8 + 2 * i]) * inv,
-                                                     __uint_as_float(o[q * 8 + 2 * i + 1]) * inv);
-            w[i] = *reinterpret_cast<uint32_t*>(&b);
-          }
-          *reinterpret_cast<uint4*>(dst + q * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kAttTmemCols);
+  // warpgroup wg: query rows [64 wg, 64 wg + 64) of the tile; this thread holds rows r_lo = 16 (warp % 4) + lane / 4
+  // and r_lo + 8, key / feature columns 8 c + 2 (lane % 4) + {0, 1}
+  const int wg = warp >> 2;
+  const uint32_t q_addr = smem_u32(sQ) + wg * 64 * 128;
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  mbar_wait(bar_q, 0);
+  for (int j = 0; j < n_blk; ++j) {
+    const int st = j & 1;
+    const uint32_t ph = (j >> 1) & 1;
+    mbar_wait(&bar_k_full[st], ph);
+    float s[32];
+    const uint32_t k_addr = smem_u32(sK + st * kAttKVBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < kAttDH / 16; ++ks)
+      wgmma_m64n64k16_ss(s, wgmma_desc_sw128(q_addr + ks * 32), wgmma_desc_sw128(k_addr + ks * 32), ks > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+
+    const int kbase = j * kAttBN + 2 * (lane & 3);
+    if (j * kAttBN + kAttBN > L) {  // only the last block of a sequence whose length is not a multiple of 64
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (kbase + 8 * c + e >= L) s[4 * c + e] = s[4 * c + 2 + e] = -INFINITY;  // exp2 -> 0, never the max
+    }
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) mx = fmaxf(mx, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx * scale_log2e);  // finite: >= 1 valid key per block
+      alpha[h] = att_exp2(m_run[h] - m_new);                 // first block: exp2(-inf) = 0
+      m_run[h] = m_new;
+    }
+    // p = exp2(s * scale - m), packed straight into the A fragment of P V (k-slice kk = keys 16 kk .. 16 kk + 15)
+    uint32_t pa[4][4];
+    float rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float p0 = att_exp2(fmaf(s[4 * c + 2 * h], scale_log2e, -m_run[h]));
+        const float p1 = att_exp2(fmaf(s[4 * c + 2 * h + 1], scale_log2e, -m_run[h]));
+        rs[h] += p0 + p1;
+        pa[c >> 1][(c & 1) * 2 + h] = att_pack_bf16x2(p0, p1);
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + rs[h];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      o[4 * c + 0] *= alpha[0];
+      o[4 * c + 1] *= alpha[0];
+      o[4 * c + 2] *= alpha[1];
+      o[4 * c + 3] *= alpha[1];
+    }
+    mbar_wait(&bar_v_full[st], ph);
+    const uint32_t v_addr = smem_u32(sV + st * kAttKVBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kAttBN / 16; ++kk)
+      wgmma_m64n64k16_rs_bmn(o, pa[kk], wgmma_desc_sw128(v_addr + kk * 16 * 128), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bar_kv_empty[st]);
+  }
+
+  // epilogue: O / l -> bf16 -> ctx[start + row, head*64 .. +64)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.f / l;
+    const int row = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    if (row < L) {
+      __nv_bfloat16* dst = ctx + int64_t(start + row) * H + head * kAttDH + 2 * (lane & 3);
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        *reinterpret_cast<uint32_t*>(dst + 8 * c) = att_pack_bf16x2(o[4 * c + 2 * h] * inv, o[4 * c + 2 * h + 1] * inv);
+    }
+  }
 }
 
 int launch_attention_tc(const void* qkv, const int32_t* cu_seqlens, int n_seqs, int total_tokens, int max_len, int H,

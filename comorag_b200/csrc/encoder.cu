@@ -2,7 +2,7 @@
 // (BGEEmbedding.py:119-127: BertModel forward -> mean_pooling -> F.normalize)
 // as one stream-ordered launch sequence over a packed (unpadded) token batch.
 // Post-LN BERT layer, exactly HF's BertLayer:
-//   qkv  = x Wqkv^T + b                      (tcgen05 GEMM, fused q/k/v weights)
+//   qkv  = x Wqkv^T + b                      (wgmma GEMM, fused q/k/v weights)
 //   ctx  = softmax(q k^T / sqrt(dh)) v       (varlen attention)
 //   x    = LN(ctx Wo^T + bo + x)             (GEMM + residual epilogue, LN kernel)
 //   x    = LN(gelu(x W1^T + b1) W2^T + b2 + x)
@@ -79,7 +79,7 @@ int run_layers(const crag_encoder* model, const int32_t* token_ids, const int32_
     const crag_encoder_layer& w = model->layers[l];
     rc = gemm_bf16(b.x, H, w.w_qkv, H, w.b_qkv, nullptr, 0, b.qkv, 3 * H, T, 3 * H, H, GEMM_EPI_BIAS, stream);
     if (rc != CRAG_OK) return rc;
-    // head dim 64 (bge-base / bge-large): tcgen05 kernel; head dim 32 (bge-small): mma.sync kernel
+    // head dim 64 (bge-base / bge-large): wgmma kernel; head dim 32 (bge-small): mma.sync kernel
     rc = (H / model->heads == 64)
              ? launch_attention_tc(b.qkv, cu_seqlens, n_seqs, T, max_seqlen, H, model->heads, b.ctx, stream)
              : launch_attention(b.qkv, cu_seqlens, n_seqs, max_seqlen, H, model->heads, b.ctx, stream);

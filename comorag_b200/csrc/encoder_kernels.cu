@@ -14,7 +14,7 @@
 //   attention         varlen multi-head self-attention, flash-style online
 //                     softmax, mma.sync m16n8k16 bf16 tiles: head dim 32
 //                     (bge-small) only -- head dim 64 runs attention_tc.cu on
-//                     tcgen05
+//                     wgmma
 //   pool_normalize    K3: masked mean over tokens + L2 normalise, writes fp32
 //                     [n, H] for the host API and (optionally) the bf16 row
 //                     straight into the corpus shard

@@ -1,17 +1,17 @@
-// K1: bf16 x bf16 -> fp32 GEMM on tcgen05 tensor cores with fused epilogues, the
-// dense contractions of the encoder forward the reference runs through
+// K1: bf16 x bf16 -> fp32 GEMM on Hopper wgmma tensor cores with fused epilogues,
+// the dense contractions of the encoder forward the reference runs through
 // `self.embedding_model(**inputs)` (BGEEmbedding.py:120): QKV, attention-output,
 // FFN-up (+GELU) and FFN-down projections of every BERT layer.
 //
 //   out[M, N] = epilogue( A[M, K] . W[N, K]^T + bias[N] )      (torch Linear layout)
 //
-// Persistent CTAs (one per SM, 192 threads):
-//   warp 0   TMA producer   A box 128x64, W box BNx64 (128-byte swizzle), STAGES ring
-//   warp 1   tcgen05.mma issuer, UMMA 128 x BN x 16, fp32 accumulators in TMEM,
-//            two accumulator buffers (2*BN columns) so tile i+1's MMAs overlap
-//            tile i's epilogue
-//   warps 2-5  epilogue: tcgen05.ld 32 columns at a time, +bias, optional exact
-//            GELU or residual add, round to bf16, 16-byte global stores
+// One CTA per 128 x 128 output tile, two CTAs per SM (288 threads each):
+//   warps 0-7  two consumer warpgroups, 64 rows each: wgmma m64n128k16 from the
+//              swizzled smem stages into fp32 register accumulators, then the
+//              epilogue (+bias, optional exact GELU or residual add, bf16 stores)
+//   warp 8     TMA producer: A box 128x64, W box 128x64 (128-byte swizzle)
+//              through a STAGES-deep mbarrier ring
+// With two CTAs resident, one CTA's epilogue overlaps the other's main loop.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -21,15 +21,18 @@
 namespace crag {
 
 constexpr int kGemmBM = 128;
+constexpr int kGemmBN = 128;
 constexpr int kGemmBK = 64;
-constexpr int kGemmThreads = 192;
+constexpr int kGemmConsumerWarps = 8;
+constexpr int kGemmThreads = 32 * kGemmConsumerWarps + 32;
+// 3 stages of 32 KB: two CTAs (2 x 97 KB) fit in an SM's 228 KB of shared memory
+constexpr int kGemmStages = 3;
 
-template <int BN, int STAGES>
 struct GemmLayout {
   static constexpr int kABytes = kGemmBM * kGemmBK * 2;  // 16 KB
-  static constexpr int kBBytes = BN * kGemmBK * 2;
+  static constexpr int kBBytes = kGemmBN * kGemmBK * 2;  // 16 KB
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr size_t smem_bytes() { return 1024 + size_t(STAGES) * kStageBytes + (2 * STAGES + 4) * 8 + 16; }
+  static constexpr size_t smem_bytes() { return 1024 + size_t(kGemmStages) * kStageBytes + 2 * kGemmStages * 8; }
 };
 
 // Exact-erf GELU (HF "gelu"), erf by Abramowitz-Stegun 7.1.26 (|abs err| <= 1.5e-7, far below the bf16 output's
@@ -52,557 +55,149 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaf(half_x, copysignf(erf_abs, z), half_x);  // 0.5 x (1 + erf(z))
 }
 
-// Packed fp32x2 arithmetic (Blackwell FFMA2 / FMUL2 / FADD2): two lanes per instruction, which halves the FMA-pipe
-// instruction count of the GELU polynomial in the issue-bound FFN-up epilogue.
-__device__ __forceinline__ uint64_t f2_pack(float a, float b) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(uint64_t v, float& a, float& b) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_splat(float a) { return f2_pack(a, a); }
-
-// gelu_erf on a pair (same A&S 7.1.26 erf as the scalar version)
-__device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
-  const uint64_t x = f2_pack(x0, x1);
-  const uint64_t z = f2_mul(x, f2_splat(0.70710678118654752f));
-  float z0, z1;
-  f2_unpack(z, z0, z1);
-  const uint64_t az = f2_pack(fabsf(z0), fabsf(z1));
-  float d0, d1;
-  f2_unpack(f2_fma(az, f2_splat(0.3275911f), f2_splat(1.0f)), d0, d1);
-  float t0, t1;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t0) : "f"(d0));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t1) : "f"(d1));
-  const uint64_t t = f2_pack(t0, t1);
-  uint64_t p = f2_fma(f2_splat(1.061405429f), t, f2_splat(-1.453152027f));
-  p = f2_fma(p, t, f2_splat(1.421413741f));
-  p = f2_fma(p, t, f2_splat(-0.284496736f));
-  p = f2_fma(p, t, f2_splat(0.254829592f));
-  p = f2_mul(p, t);
-  float a0, a1;
-  f2_unpack(f2_mul(f2_mul(az, az), f2_splat(-1.4426950408889634f)), a0, a1);
-  float e0, e1;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(a0));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
-  // erf(|z|) = 1 - p * e ; result = 0.5 x (1 + sign(z) erf(|z|))
-  float r0, r1;
-  f2_unpack(f2_fma(f2_mul(p, f2_splat(-1.0f)), f2_pack(e0, e1), f2_splat(1.0f)), r0, r1);
-  const uint64_t half_x = f2_mul(x, f2_splat(0.5f));
-  f2_unpack(f2_fma(half_x, f2_pack(copysignf(r0, z0), copysignf(r1, z1)), half_x), x0, x1);
-}
-
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-
-// bias (+GELU | +residual) on 32 consecutive fp32 accumulator columns of one output row, bf16 16-byte stores
 template <int EPI>
-__device__ __forceinline__ void epilogue_chunk(const uint32_t (&r)[32], int row, int col0, int M, int N,
-                                               const float* __restrict__ bias,
-                                               const __nv_bfloat16* __restrict__ residual, int64_t ldr,
-                                               __nv_bfloat16* __restrict__ out, int64_t ldo) {
-  if (row >= M || col0 >= N) return;
-  __nv_bfloat16* orow = out + int64_t(row) * ldo + col0;
-  const __nv_bfloat16* rrow = (EPI == GEMM_EPI_BIAS_RESIDUAL) ? residual + int64_t(row) * ldr + col0 : nullptr;
-#pragma unroll
-  for (int v = 0; v < 4; ++v) {  // 8 columns (16 bytes) per store
-    if (col0 + v * 8 < N) {
-      float x[8];
-      const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + col0 + v * 8));
-      const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias + col0 + v * 8 + 4));
-      x[0] = __uint_as_float(r[v * 8 + 0]) + b0.x;
-      x[1] = __uint_as_float(r[v * 8 + 1]) + b0.y;
-      x[2] = __uint_as_float(r[v * 8 + 2]) + b0.z;
-      x[3] = __uint_as_float(r[v * 8 + 3]) + b0.w;
-      x[4] = __uint_as_float(r[v * 8 + 4]) + b1.x;
-      x[5] = __uint_as_float(r[v * 8 + 5]) + b1.y;
-      x[6] = __uint_as_float(r[v * 8 + 6]) + b1.z;
-      x[7] = __uint_as_float(r[v * 8 + 7]) + b1.w;
-      if (EPI == GEMM_EPI_BIAS_GELU) {
-#pragma unroll
-        for (int j = 0; j < 8; j += 2) gelu_erf2(x[j], x[j + 1]);
-      }
-      if (EPI == GEMM_EPI_BIAS_RESIDUAL) {
-        const uint4 rv = *reinterpret_cast<const uint4*>(rrow + v * 8);
-        const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const __nv_bfloat162 p = *reinterpret_cast<const __nv_bfloat162*>(&rw[j]);
-          x[2 * j] += __bfloat162float(p.x);
-          x[2 * j + 1] += __bfloat162float(p.y);
-        }
-      }
-      uint4 o;
-      o.x = pack_bf16x2(x[0], x[1]);
-      o.y = pack_bf16x2(x[2], x[3]);
-      o.z = pack_bf16x2(x[4], x[5]);
-      o.w = pack_bf16x2(x[6], x[7]);
-      *reinterpret_cast<uint4*>(orow + v * 8) = o;
-    }
-  }
-}
-
-// Same epilogue, but the bf16 chunk goes through a per-warp shared-memory staging tile first so that the global
-// stores are row-coalesced: thread = row produces 4 x 16 B of its own row (stored at pitch 80 B, conflict-free for
-// quarter-warps); then 4 lanes cover one row's 64 B and one warp instruction writes 8 rows x 64 contiguous bytes
-// (full 32-byte sectors) instead of 32 rows x 16 B.  `stage` is this warp's private 32 x 80 B tile.
-constexpr int kEpiStagePitch = 80;
-constexpr int kEpiStageBytes = 32 * kEpiStagePitch;
-template <int EPI>
-__device__ __forceinline__ void epilogue_chunk_staged(const uint32_t (&r)[32], int row, int row_base, int col0, int M,
-                                                      int N, const float* __restrict__ bias,
-                                                      const __nv_bfloat16* __restrict__ residual, int64_t ldr,
-                                                      __nv_bfloat16* __restrict__ out, int64_t ldo, uint8_t* stage,
-                                                      int lane) {
-  if (col0 >= N) return;  // warp-uniform
-  const bool row_ok = row < M;
-  const __nv_bfloat16* rrow = (EPI == GEMM_EPI_BIAS_RESIDUAL) ? residual + int64_t(row) * ldr + col0 : nullptr;
-#pragma unroll
-  for (int v = 0; v < 4; ++v) {
-    uint4 o = make_uint4(0u, 0u, 0u, 0u);
-    if (col0 + v * 8 < N) {
-      float x[8];
-      const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + col0 + v * 8));
-      const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias + col0 + v * 8 + 4));
-      x[0] = __uint_as_float(r[v * 8 + 0]) + b0.x;
-      x[1] = __uint_as_float(r[v * 8 + 1]) + b0.y;
-      x[2] = __uint_as_float(r[v * 8 + 2]) + b0.z;
-      x[3] = __uint_as_float(r[v * 8 + 3]) + b0.w;
-      x[4] = __uint_as_float(r[v * 8 + 4]) + b1.x;
-      x[5] = __uint_as_float(r[v * 8 + 5]) + b1.y;
-      x[6] = __uint_as_float(r[v * 8 + 6]) + b1.z;
-      x[7] = __uint_as_float(r[v * 8 + 7]) + b1.w;
-      if (EPI == GEMM_EPI_BIAS_GELU) {
-#pragma unroll
-        for (int j = 0; j < 8; j += 2) gelu_erf2(x[j], x[j + 1]);
-      }
-      if (EPI == GEMM_EPI_BIAS_RESIDUAL) {
-        if (row_ok) {
-          const uint4 rv = *reinterpret_cast<const uint4*>(rrow + v * 8);
-          const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const __nv_bfloat162 p = *reinterpret_cast<const __nv_bfloat162*>(&rw[j]);
-            x[2 * j] += __bfloat162float(p.x);
-            x[2 * j + 1] += __bfloat162float(p.y);
-          }
-        }
-      }
-      o.x = pack_bf16x2(x[0], x[1]);
-      o.y = pack_bf16x2(x[2], x[3]);
-      o.z = pack_bf16x2(x[4], x[5]);
-      o.w = pack_bf16x2(x[6], x[7]);
-    }
-    *reinterpret_cast<uint4*>(stage + lane * kEpiStagePitch + v * 16) = o;
-  }
-  __syncwarp();
-  const int piece = lane & 3;
-  const int gcol = col0 + piece * 8;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r2 = i * 8 + (lane >> 2);
-    const int grow = row_base + r2;
-    if (grow < M && gcol < N)
-      *reinterpret_cast<uint4*>(out + int64_t(grow) * ldo + gcol) =
-          *reinterpret_cast<const uint4*>(stage + r2 * kEpiStagePitch + piece * 16);
-  }
-  __syncwarp();  // the staging tile is reused by the next chunk
-}
-
-template <int BN, int STAGES, int EPI>
-__global__ void __launch_bounds__(kGemmThreads, 1)
+__global__ void __launch_bounds__(kGemmThreads, 2)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, int M, int N,
                  int K, const float* __restrict__ bias, const __nv_bfloat16* __restrict__ residual, int64_t ldr,
                  __nv_bfloat16* __restrict__ out, int64_t ldo) {
-  using L = GemmLayout<BN, STAGES>;
+  using L = GemmLayout;
+  constexpr int STAGES = kGemmStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * L::kStageBytes);
   uint64_t* bar_empty = bar_full + STAGES;
-  uint64_t* bar_tfull = bar_empty + STAGES;  // [2]
-  uint64_t* bar_tempty = bar_tfull + 2;      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_tempty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int m_tiles = (M + kGemmBM - 1) / kGemmBM;
-  const int n_tiles = (N + BN - 1) / BN;
-  const int num_tiles = m_tiles * n_tiles;
+  const int n_blk = blockIdx.x, m_blk = blockIdx.y;
   const int num_kb = (K + kGemmBK - 1) / kGemmBK;
-  constexpr uint32_t kTmemCols = 2 * BN;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_a);
-    tma_prefetch_desc(&tm_b);
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&bar_full[s], 1);
-      mbar_init(&bar_empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&bar_tfull[a], 1);
-      mbar_init(&bar_tempty[a], 4);
+      mbar_init(&bar_empty[s], kGemmConsumerWarps);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (warp == kGemmConsumerWarps) {
+    // ================================================================ producer
+    if (lane == 0) {
+      tma_prefetch_desc(&tm_a);
+      tma_prefetch_desc(&tm_b);
       const uint64_t pol_w = policy_evict_last();
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&bar_empty[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * L::kStageBytes;
-          mbar_arrive_expect_tx(&bar_full[stage], L::kStageBytes);
-          tma_load_2d(&tm_a, &bar_full[stage], sa, kb * kGemmBK, m_blk * kGemmBM);
-          tma_load_2d_hint(&tm_b, &bar_full[stage], sa + L::kABytes, kb * kGemmBK, n_blk * BN, pol_w);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&bar_empty[stage], phase ^ 1);
+        uint8_t* sa = smem + stage * L::kStageBytes;
+        mbar_arrive_expect_tx(&bar_full[stage], L::kStageBytes);
+        tma_load_2d(&tm_a, &bar_full[stage], sa, kb * kGemmBK, m_blk * kGemmBM);
+        tma_load_2d_hint(&tm_b, &bar_full[stage], sa + L::kABytes, kb * kGemmBK, n_blk * kGemmBN, pol_w);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(kGemmBM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&bar_tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&bar_full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
-          const uint32_t b_addr = a_addr + L::kABytes;
-#pragma unroll
-          for (int ks = 0; ks < kGemmBK / 16; ++ks)
-            umma_f16(d_tmem, umma_desc_k_sw128(a_addr + ks * 32), umma_desc_k_sw128(b_addr + ks * 32), idesc,
-                     (kb | ks) != 0);
-          umma_commit(&bar_empty[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&bar_tfull[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else {
-    const int quad = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
-      const int row = m_blk * kGemmBM + quad * 32 + lane;
-      const int n0 = n_blk * BN;
-      mbar_wait(&bar_tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + (uint32_t(quad * 32) << 16) + acc * BN;
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(t_addr + c * 32, r);
-        tmem_ld_wait();
-        epilogue_chunk<EPI>(r, row, n0 + c * 32, M, N, bias, residual, ldr, out, ldo);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_tempty[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
+  // ================================================ consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile
+  const int wg = warp >> 2;
+  float acc[kGemmBN / 2];
+#pragma unroll
+  for (int i = 0; i < kGemmBN / 2; ++i) acc[i] = 0.f;
+  int stage = 0, prev = 0;
+  uint32_t phase = 0;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&bar_full[stage], phase);
+    const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes) + wg * 64 * 128;
+    const uint32_t b_addr = smem_u32(smem + stage * L::kStageBytes + L::kABytes);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < kGemmBK / 16; ++ks)
+      wgmma_m64n128k16_ss(acc, wgmma_desc_sw128(a_addr + ks * 32), wgmma_desc_sw128(b_addr + ks * 32), 1u);
+    wgmma_commit();
+    wgmma_wait<1>();  // k-block kb - 1 has retired: its stage goes back to the producer
+    if (kb > 0 && lane == 0) mbar_arrive(&bar_empty[prev]);
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+
+  // epilogue: bias (+GELU | +residual), bf16 pairs straight from the accumulator fragment
+  const int row0 = m_blk * kGemmBM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int col0 = n_blk * kGemmBN + 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < kGemmBN / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= N) continue;
+    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      if (row >= M) continue;
+      float x0 = acc[4 * j + 2 * h] + b.x, x1 = acc[4 * j + 2 * h + 1] + b.y;
+      if (EPI == GEMM_EPI_BIAS_GELU) {
+        x0 = gelu_erf(x0);
+        x1 = gelu_erf(x1);
+      }
+      if (EPI == GEMM_EPI_BIAS_RESIDUAL) {
+        const __nv_bfloat162 r = *reinterpret_cast<const __nv_bfloat162*>(residual + int64_t(row) * ldr + col);
+        x0 += __bfloat162float(r.x);
+        x1 += __bfloat162float(r.y);
+      }
+      *reinterpret_cast<uint32_t*>(out + int64_t(row) * ldo + col) = pack_bf16x2(x0, x1);
+    }
+  }
 }
 
-template <int BN, int STAGES, int EPI>
+template <int EPI>
 static int launch_gemm_t(const CUtensorMap& tm_a, const CUtensorMap& tm_b, int M, int N, int K, const float* bias,
                          const __nv_bfloat16* residual, int64_t ldr, __nv_bfloat16* out, int64_t ldo,
                          cudaStream_t stream) {
-  using L = GemmLayout<BN, STAGES>;
-  auto kern = gemm_bf16_kernel<BN, STAGES, EPI>;
-  CRAG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(L::smem_bytes())));
-  const int tiles = ((M + kGemmBM - 1) / kGemmBM) * ((N + BN - 1) / BN);
-  int grid = sm_count();
-  if (grid <= 0) grid = 148;
-  if (tiles < grid) grid = tiles;
-  kern<<<grid, kGemmThreads, L::smem_bytes(), stream>>>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo);
-  CRAG_CUDA_OK(cudaGetLastError());
-  return CRAG_OK;
-}
-
-template <int BN, int STAGES>
-static int launch_gemm_e(int epi, const CUtensorMap& tm_a, const CUtensorMap& tm_b, int M, int N, int K,
-                         const float* bias, const __nv_bfloat16* residual, int64_t ldr, __nv_bfloat16* out,
-                         int64_t ldo, cudaStream_t stream) {
-  switch (epi) {
-    case GEMM_EPI_BIAS: return launch_gemm_t<BN, STAGES, GEMM_EPI_BIAS>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo, stream);
-    case GEMM_EPI_BIAS_GELU: return launch_gemm_t<BN, STAGES, GEMM_EPI_BIAS_GELU>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo, stream);
-    case GEMM_EPI_BIAS_RESIDUAL: return launch_gemm_t<BN, STAGES, GEMM_EPI_BIAS_RESIDUAL>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo, stream);
-  }
-  return fail(CRAG_ERR_INVALID, "gemm: unknown epilogue %d", epi);
-}
-
-
-// ---------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2): a cluster of two CTAs owns a 256 x BN output tile.  Each CTA TMA-loads its own
-// 128 rows of A and HALF of the W tile (BN/2 rows); the leader's single tcgen05.mma.cta_group::2 reads both CTAs'
-// shared memory and accumulates rows 0-127 into the leader's TMEM and rows 128-255 into the peer's.  L2->SM traffic
-// per flop drops by 1/3 against the 128 x 256 single-CTA tile (the W tile is fetched once per pair), which is what
-// bounds the single-CTA kernel.  EPI_WARPS = 4 or 8 (8: two warps per TMEM lane quadrant, half the columns each).
-template <int BN, int STAGES>
-struct Gemm2Layout {
-  static constexpr int kABytes = 128 * kGemmBK * 2;         // this CTA's 128 rows of A
-  static constexpr int kBBytes = (BN / 2) * kGemmBK * 2;    // this CTA's half of the W tile
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr size_t kBarBytes = 256;  // (2*STAGES + 4) mbarriers + the TMEM slot, rounded up
-  static constexpr size_t smem_bytes(int epi_warps) {
-    return 1024 + size_t(STAGES) * kStageBytes + kBarBytes + size_t(epi_warps) * kEpiStageBytes;
-  }
-};
-
-// EPI_WARPS = 16 (four warps per lane quadrant, 64 columns each) is used for the GELU epilogue, which is issue-bound:
-// measured on B200 at M=16384, N=4096, K=1024: 1138 -> 1262 TFLOP/s; the residual epilogue gains nothing from it.
-// (A software-pipelined epilogue -- next tcgen05.ld and residual rows in flight during the current chunk -- was
-// measured in round 2 and removed: no gain at K=4096, 12 % slower at N=K=1024.)
-template <int BN, int STAGES, int EPI, int EPI_WARPS>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(64 + 32 * EPI_WARPS, 1)
-gemm2_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, int M, int N,
-                  int K, const float* __restrict__ bias, const __nv_bfloat16* __restrict__ residual, int64_t ldr,
-                  __nv_bfloat16* __restrict__ out, int64_t ldo) {
-  using L = Gemm2Layout<BN, STAGES>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * L::kStageBytes);
-  uint64_t* bar_empty = bar_full + STAGES;
-  uint64_t* bar_tfull = bar_empty + STAGES;  // [2]
-  uint64_t* bar_tempty = bar_tfull + 2;      // [2]  (used in the leader only)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_tempty + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t cta = cluster_ctarank();
-  const bool leader = cta == 0;
-  const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
-  const int m_tiles = (M + 255) / 256;
-  const int n_tiles = (N + BN - 1) / BN;
-  const int num_tiles = m_tiles * n_tiles;
-  const int num_kb = (K + kGemmBK - 1) / kGemmBK;
-  constexpr uint32_t kTmemCols = 2 * BN;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_a);
-    tma_prefetch_desc(&tm_b);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&bar_full[s], 1);   // leader: one arrive.expect_tx, bytes from both CTAs' TMA
-      mbar_init(&bar_empty[s], 1);  // multicast tcgen05.commit from the leader
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&bar_tfull[a], 1);
-      mbar_init(&bar_tempty[a], 2 * EPI_WARPS);  // every epilogue warp of both CTAs
-    }
-    fence_mbar_init();
-  }
-  if (warp == 1) {
-    tmem_alloc_2cta(tmem_slot, kTmemCols);
-    tmem_relinquish_2cta();
-  }
-  tc_fence_before();
-  cluster_sync_all();   // both CTAs' barriers initialised and TMEM allocated before any cross-CTA traffic
-  __syncthreads();      // (the cluster barrier already orders this; the CTA barrier keeps racecheck's model happy)
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      // measured: evict_first on the activation stream beats evict_normal by 3-8 % (W stays resident with evict_last)
-      const uint64_t pol_a = policy_evict_first(), pol_w = policy_evict_last();
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&bar_empty[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * L::kStageBytes;
-          if (leader) mbar_arrive_expect_tx(&bar_full[stage], 2 * L::kStageBytes);
-          tma_load_2d_2cta(&tm_a, &bar_full[stage], sa, kb * kGemmBK, m_blk * 256 + int(cta) * 128, pol_a);
-          tma_load_2d_2cta(&tm_b, &bar_full[stage], sa + L::kABytes, kb * kGemmBK, n_blk * BN + int(cta) * (BN / 2), pol_w);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (leader && elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(256, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        mbar_wait(&bar_tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&bar_full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
-          const uint32_t b_addr = a_addr + L::kABytes;
-#pragma unroll
-          for (int ks = 0; ks < kGemmBK / 16; ++ks)
-            umma_f16_2cta(d_tmem, umma_desc_k_sw128(a_addr + ks * 32), umma_desc_k_sw128(b_addr + ks * 32), idesc,
-                          (kb | ks) != 0);
-          umma_commit_2cta_mc(&bar_empty[stage], 3);  // frees the slot in both CTAs
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2cta_mc(&bar_tfull[acc], 3);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else {
-    const int quad = warp & 3;
-    uint8_t* stage = smem + STAGES * L::kStageBytes + L::kBarBytes + (warp - 2) * kEpiStageBytes;
-    constexpr int kColsPerWarp = BN / (EPI_WARPS / 4);
-    const int col_begin = ((warp - 2) >> 2) * kColsPerWarp;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-      const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
-      const int row_base = m_blk * 256 + int(cta) * 128 + quad * 32;
-      const int row = row_base + lane;
-      const int n0 = n_blk * BN + col_begin;
-      mbar_wait(&bar_tfull[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + (uint32_t(quad * 32) << 16) + acc * BN + col_begin;
-#pragma unroll 1
-      for (int c = 0; c < kColsPerWarp / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(t_addr + c * 32, r);
-        tmem_ld_wait();
-        epilogue_chunk_staged<EPI>(r, row, row_base, n0 + c * 32, M, N, bias, residual, ldr, out, ldo, stage, lane);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(&bar_tempty[acc]);
-        else mbar_arrive_remote(&bar_tempty[acc], 0);
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();  // the peer's smem/TMEM stay alive until the leader's last MMA has been consumed
-  if (warp == 1) tmem_dealloc_2cta(tmem_base, kTmemCols);
-}
-
-template <int BN, int STAGES, int EPI, int EPI_WARPS>
-static int launch_gemm2_t(const CUtensorMap& tm_a, const CUtensorMap& tm_b, int M, int N, int K, const float* bias,
-                          const __nv_bfloat16* residual, int64_t ldr, __nv_bfloat16* out, int64_t ldo,
-                          cudaStream_t stream) {
-  using L = Gemm2Layout<BN, STAGES>;
-  auto kern = gemm2_bf16_kernel<BN, STAGES, EPI, EPI_WARPS>;
+  auto kern = gemm_bf16_kernel<EPI>;
   {  // once per kernel and device, not per launch
     static bool done[64] = {false};
     int dev = 0;
     CRAG_CUDA_OK(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64 || !done[dev]) {
-      CRAG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(L::smem_bytes(EPI_WARPS))));
+      CRAG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(GemmLayout::smem_bytes())));
       if (dev >= 0 && dev < 64) done[dev] = true;
     }
   }
-  const int tiles = ((M + 255) / 256) * ((N + BN - 1) / BN);
-  int sms = sm_count();
-  if (sms <= 0) sms = 148;
-  int pairs = sms / 2;
-  if (tiles < pairs) pairs = tiles;
-  kern<<<2 * pairs, 64 + 32 * EPI_WARPS, L::smem_bytes(EPI_WARPS), stream>>>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo);
+  const dim3 grid((N + kGemmBN - 1) / kGemmBN, (M + kGemmBM - 1) / kGemmBM);
+  kern<<<grid, kGemmThreads, GemmLayout::smem_bytes(), stream>>>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }
 
-template <int BN, int STAGES>
-static int launch_gemm2_e(int epi, const CUtensorMap& tm_a, const CUtensorMap& tm_b, int M, int N, int K,
-                          const float* bias, const __nv_bfloat16* residual, int64_t ldr, __nv_bfloat16* out,
-                          int64_t ldo, cudaStream_t stream) {
-  switch (epi) {
-    case GEMM_EPI_BIAS: return launch_gemm2_t<BN, STAGES, GEMM_EPI_BIAS, 4>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo, stream);
-    case GEMM_EPI_BIAS_GELU: return launch_gemm2_t<BN, STAGES, GEMM_EPI_BIAS_GELU, 8>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo, stream);
-    case GEMM_EPI_BIAS_RESIDUAL: return launch_gemm2_t<BN, STAGES, GEMM_EPI_BIAS_RESIDUAL, 8>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo, stream);
-  }
-  return fail(CRAG_ERR_INVALID, "gemm: unknown epilogue %d", epi);
-}
-
 int gemm_bf16(const void* a, int64_t lda, const void* w, int64_t ldw, const float* bias, const void* residual,
-              int64_t ldr, void* out, int64_t ldo, int M, int N, int K, int epi, cudaStream_t stream, int variant) {
+              int64_t ldr, void* out, int64_t ldo, int M, int N, int K, int epi, cudaStream_t stream) {
   if (M <= 0) return CRAG_OK;
-  // A/B testing of whole forwards: CRAG_GEMM_VARIANT=<bits> applies a variant word to every GEMM that did not ask for
-  // one (read once; unset = the default dispatch).  Not a tuning knob for production use.
-  static const int env_variant = [] { const char* e = getenv("CRAG_GEMM_VARIANT"); return e ? atoi(e) : 0; }();
-  if (variant == 0) variant = env_variant;
   if (N < 8 || K < 8 || N % 8 != 0 || K % 8 != 0) return fail(CRAG_ERR_INVALID, "gemm: N and K must be positive multiples of 8 (N=%d K=%d)", N, K);
   if (lda % 8 || ldw % 8 || ldo % 8 || (epi == GEMM_EPI_BIAS_RESIDUAL && ldr % 8)) return fail(CRAG_ERR_INVALID, "gemm: leading dimensions must be multiples of 8 elements");
   if (!a || !w || !bias || !out || (epi == GEMM_EPI_BIAS_RESIDUAL && !residual)) return fail(CRAG_ERR_INVALID, "gemm: null pointer");
   if ((uintptr_t(a) | uintptr_t(w) | uintptr_t(out) | uintptr_t(bias) | uintptr_t(residual)) & 15) return fail(CRAG_ERR_INVALID, "gemm: pointers must be 16-byte aligned");
-  bool wide = (N % 256 == 0) || N >= 1024;
-  if (variant & 2) wide = false;  // A/B switch: force the BN = 128 tile
-  // Short batches (the query side: a wave of <= 32 probes is a few hundred tokens): a 256 x 256 pair tile leaves
-  // most SMs idle and serialises the whole K loop on a handful of CTAs (FFN-down at M = 768: 12 pair tiles x 64
-  // k-blocks).  128 x 128 single-CTA tiles give 4x the CTAs and a K loop per CTA that is half as long.
-  static const int small_m = [] { const char* e = getenv("CRAG_GEMM_SMALL_M"); return e ? atoi(e) : 1024; }();
-  if (M <= small_m && !(variant & 8)) {
-    variant |= 1;
-    wide = false;
-  }
+  if ((M + kGemmBM - 1) / kGemmBM > 65535) return fail(CRAG_ERR_INVALID, "gemm: M too large (%d)", M);
   const __nv_bfloat16* res = static_cast<const __nv_bfloat16*>(residual);
   __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out);
   CUtensorMap tm_a, tm_b;
   int rc = make_tmap_bf16_2d(&tm_a, a, uint64_t(M), uint64_t(K), uint64_t(lda) * 2, kGemmBM);
   if (rc != CRAG_OK) return rc;
-  if (M > 128 && !(variant & 1)) {
-    // CTA-pair kernel: each CTA fetches half of the W tile
-    rc = make_tmap_bf16_2d(&tm_b, w, uint64_t(N), uint64_t(K), uint64_t(ldw) * 2, wide ? 128 : 64);
-    if (rc != CRAG_OK) return rc;
-    // GELU epilogue on the wide tile: 16 epilogue warps, one pipeline stage traded for their staging tiles
-    if (wide && epi == GEMM_EPI_BIAS_GELU && !(variant & 4))
-      return launch_gemm2_t<256, 5, GEMM_EPI_BIAS_GELU, 16>(tm_a, tm_b, M, N, K, bias, res, ldr, o, ldo, stream);
-    if (wide) return launch_gemm2_e<256, 6>(epi, tm_a, tm_b, M, N, K, bias, res, ldr, o, ldo, stream);
-    return launch_gemm2_e<128, 8>(epi, tm_a, tm_b, M, N, K, bias, res, ldr, o, ldo, stream);
-  }
-  rc = make_tmap_bf16_2d(&tm_b, w, uint64_t(N), uint64_t(K), uint64_t(ldw) * 2, wide ? 256 : 128);
+  rc = make_tmap_bf16_2d(&tm_b, w, uint64_t(N), uint64_t(K), uint64_t(ldw) * 2, kGemmBN);
   if (rc != CRAG_OK) return rc;
-  if (wide) return launch_gemm_e<256, 4>(epi, tm_a, tm_b, M, N, K, bias, res, ldr, o, ldo, stream);
-  return launch_gemm_e<128, 6>(epi, tm_a, tm_b, M, N, K, bias, res, ldr, o, ldo, stream);
+  switch (epi) {
+    case GEMM_EPI_BIAS: return launch_gemm_t<GEMM_EPI_BIAS>(tm_a, tm_b, M, N, K, bias, res, ldr, o, ldo, stream);
+    case GEMM_EPI_BIAS_GELU: return launch_gemm_t<GEMM_EPI_BIAS_GELU>(tm_a, tm_b, M, N, K, bias, res, ldr, o, ldo, stream);
+    case GEMM_EPI_BIAS_RESIDUAL: return launch_gemm_t<GEMM_EPI_BIAS_RESIDUAL>(tm_a, tm_b, M, N, K, bias, res, ldr, o, ldo, stream);
+  }
+  return fail(CRAG_ERR_INVALID, "gemm: unknown epilogue %d", epi);
 }
 
 }  // namespace crag
@@ -610,8 +205,6 @@ int gemm_bf16(const void* a, int64_t lda, const void* w, int64_t ldw, const floa
 extern "C" int crag_gemm_bf16(const void* a, int64_t lda, const void* w, int64_t ldw, const float* bias,
                               const void* residual, int64_t ldr, void* out, int64_t ldo, int m, int n, int k,
                               int epilogue, crag_stream_t stream) {
-  // bits 8+ of `epilogue` select a kernel variant for A/B measurements (tools/gpu_check_encoder.py): 0 = default
-  // dispatch, bit 0 = force single-CTA, bit 1 = force the BN = 128 tile, bit 2 = 8 (not 16) GELU epilogue warps
-  return crag::gemm_bf16(a, lda, w, ldw, bias, residual, ldr, out, ldo, m, n, k, epilogue & 0xFF,
-                         static_cast<cudaStream_t>(stream), epilogue >> 8);
+  return crag::gemm_bf16(a, lda, w, ldw, bias, residual, ldr, out, ldo, m, n, k, epilogue,
+                         static_cast<cudaStream_t>(stream));
 }

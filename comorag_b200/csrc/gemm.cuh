@@ -1,4 +1,4 @@
-// Internal interface of the tcgen05 GEMM (gemm.cu), used by the encoder driver.
+// Internal interface of the wgmma GEMM (gemm.cu), used by the encoder driver.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -15,6 +15,6 @@ enum : int {
 
 // out[M,N] (bf16) = epi(A[M,K] (bf16) . W[N,K]^T (bf16) + bias[N] (fp32)); leading dims in elements.
 int gemm_bf16(const void* a, int64_t lda, const void* w, int64_t ldw, const float* bias, const void* residual,
-              int64_t ldr, void* out, int64_t ldo, int M, int N, int K, int epi, cudaStream_t stream, int variant = 0);
+              int64_t ldr, void* out, int64_t ldo, int M, int N, int K, int epi, cudaStream_t stream);
 
 }  // namespace crag

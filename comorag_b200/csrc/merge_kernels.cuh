@@ -1,6 +1,6 @@
 // Merge kernels of the search path: the per-shard merge of the CTAs' partial lists (merge_topk_kernel) and the fused
 // finalize + cross-rank exchange + global merge of the row-sharded index (finalize_exchange_kernel).  SIMT code over
-// shared memory and, for the exchange, peer-mapped global memory with release / acquire flags -- no tcgen05, TMA or
+// shared memory and, for the exchange, peer-mapped global memory with release / acquire flags -- no wgmma, TMA or
 // mbarrier -- kept in a header so tests/warp_emu can run exactly these kernels on emulated thread blocks (one OS
 // thread per rank for the exchange) and compare every rank's answer with the merge rule stated in plain C++.
 #pragma once

@@ -1,6 +1,6 @@
 // Pooled admission floor of the shard scan (search.cu): the warp-level routines that turn the keys all CTAs have
 // published so far into a per-query floor key.  Pure SIMT code -- loads, compares, warp reductions -- with no
-// tcgen05 / TMA / mbarrier in it, kept in its own header so that tests/warp_emu can compile exactly these functions
+// wgmma / TMA / mbarrier in it, kept in its own header so that tests/warp_emu can compile exactly these functions
 // for the host (32 emulated lanes) and check the one property exactness rests on: at least k published keys are at
 // or above the floor a refresh returns, so no row with a smaller key can belong to the shard's top-k.
 #pragma once
@@ -9,7 +9,7 @@
 
 namespace crag {
 
-constexpr int kNQ = 32;         // UMMA N: queries per pass
+constexpr int kNQ = 32;         // wgmma N: queries per pass
 
 // Pooled admission floor.  Every CTA publishes its current best kPoolM KEYS per query (after each flush of that
 // query's candidate buffer) in pool[cta][m][q] (packed u64 keys, 0 = nothing yet; query-contiguous so a warp reads
@@ -145,7 +145,7 @@ __device__ __forceinline__ uint64_t pooled_kth_key(const uint64_t* __restrict__ 
   return kth_largest_key<NV>(hi, lo, k);
 }
 
-// The usual refresh (k <= 0.8 * CTAs): only each CTA's BEST key is pooled -- the k-th largest of ~148 CTA maxima is
+// The usual refresh (k <= 0.8 * CTAs): only each CTA's BEST key is pooled -- the k-th largest of ~132 CTA maxima is
 // within a factor ~1.6 in admission rate of the true k-th best of everything seen, because k < #CTAs -- and a select
 // warp bisects the floors of ALL EIGHT queries it owns at once: the eight bisections are independent, so their
 // warp reductions pipeline instead of costing one full REDUX latency per step and query (measured before: 3.3 us per

@@ -1,5 +1,5 @@
 // The kernels of the full device ranking (rank_all.cu): a stable LSD radix sort, pure SIMT integer code (shared-memory
-// histograms, a block scan, match.any ranking inside a warp) with nothing Blackwell-specific in it.  Kept in a header
+// histograms, a block scan, match.any ranking inside a warp) with nothing architecture-specific in it.  Kept in a header
 // so tests/warp_emu can run exactly these kernels on emulated thread blocks and compare the permutation with
 // std::stable_sort (descending score, ascending row on ties) -- the bit-exact contract of ComoRAG.py:965-966.
 #pragma once

@@ -6,19 +6,21 @@
 // 32 queries per pass over the shard, without ever writing the [nq, N] score
 // matrix.
 //
-// Data flow per CTA (192 threads):
-//   warp 0   TMA producer: streams the shard as 128-row x 64-col bf16 boxes
-//            (16 KB, 128-byte swizzle) through a STAGES-deep mbarrier ring; the
-//            32 x dim query block is TMA-staged once and stays in smem.
-//   warp 1   tcgen05.mma issuer: scores[128 rows, 32 queries] accumulate in
-//            TMEM (fp32) over dim/16 UMMA steps; 16 score-tile buffers (all 512
-//            TMEM columns) so the HBM stream keeps running while the select warps
-//            are busy sorting a full candidate buffer.
-//   warps 2-5  select: each thread owns one corpus row of the tile (one TMEM
-//            lane), reads its 32 scores with tcgen05.ld, updates per-query
-//            min/max in registers and offers scores that beat the query's
-//            current k-th best to a small shared candidate buffer; full
-//            buffers are bitonic-sorted in registers by one warp (topk.cuh).
+// Data flow per CTA (288 threads):
+//   warp 8   TMA producer: streams the shard as 128-row x 64-col bf16 boxes
+//            (16 KB, 128-byte swizzle), each with the 32 x 64 query slice of
+//            the same columns (4 KB, from L2), through a STAGES-deep mbarrier
+//            ring.
+//   warps 4-7  wgmma warpgroup: scores[128 rows, 32 queries] accumulate in
+//            registers (fp32, two m64n32k16 per 16-wide K step) over the tile,
+//            then go to one of kAccStages shared-memory score tiles, so the HBM
+//            stream keeps running while the select warps are busy sorting a
+//            full candidate buffer.
+//   warps 0-3  select: each thread owns one corpus row of the tile, reads its
+//            32 scores from the score tile, updates per-query min/max in
+//            registers and offers scores that beat the query's current k-th
+//            best to a small shared candidate buffer; full buffers are
+//            bitonic-sorted in registers by one warp (topk.cuh).
 //            The admission threshold is the better of the CTA's own k-th key
 //            and a floor pooled over ALL CTAs (kPoolM below).
 // The shard is read exactly once from HBM: algorithmic bytes = n_rows*dim*2.
@@ -38,6 +40,12 @@
 
 namespace crag {
 
+// the 32 scores of row `row` of a score tile (layout: score_slot) -> r[q]
+__device__ __forceinline__ void ld_score_row(const float* tile, int row, uint32_t (&r)[kNQ]) {
+#pragma unroll
+  for (int q = 0; q < kNQ; ++q) r[q] = __float_as_uint(tile[score_slot(row, q)]);
+}
+
 template <int KLIST, int CAP, int STAGES, bool IVF = false, bool SCORES = false>
 __global__ void __launch_bounds__(kSearchThreads, 1)
 search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_constant__ CUtensorMap tm_q,
@@ -45,18 +53,19 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
                    uint64_t* __restrict__ pool, uint32_t perm_mul, int perm_shift, uint64_t* __restrict__ part_keys,
                    float* __restrict__ part_minmax, const typename IvfParam<IVF, SCORES>::type ivf) {
   using L = SearchLayout<KLIST, CAP, STAGES>;
+  static_assert(L::smem_bytes() <= 227 * 1024, "stages, score tiles and candidate lists exceed 227 KB of shared memory");
+  constexpr int kAccStages = L::kAccStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
   uint8_t* stage_base = smem;
-  uint8_t* q_base = stage_base + STAGES * kStageBytes;
-  uint64_t* keys = reinterpret_cast<uint64_t*>(q_base + num_kb * kQBlockBytes);
+  float* score_tiles = reinterpret_cast<float*>(stage_base + STAGES * kStageTotalBytes);   // [kAccStages][128 * 32]
+  uint64_t* keys = reinterpret_cast<uint64_t*>(stage_base + STAGES * kStageTotalBytes + kAccStages * kScoreTileBytes);
   uint64_t* bar_full = keys + kNQ * L::kKeysPerQuery;
   uint64_t* bar_empty = bar_full + STAGES;
   uint64_t* bar_tfull = bar_empty + STAGES;            // [kAccStages]
   uint64_t* bar_tempty = bar_tfull + kAccStages;       // [kAccStages]
-  uint64_t* bar_q = bar_tempty + kAccStages;           // [1]
-  uint64_t* thr_key = bar_q + 1;              // [kNQ]
+  uint64_t* thr_key = bar_tempty + kAccStages;         // [kNQ]
   float* thr_f = reinterpret_cast<float*>(thr_key + kNQ);  // [kNQ]
   int* cnt = reinterpret_cast<int*>(thr_f + kNQ);          // [kNQ]
   float* red = reinterpret_cast<float*>(cnt + kNQ);        // [4][kNQ][2]
@@ -64,7 +73,6 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
   float* bnd_f = reinterpret_cast<float*>(bnd_key + kNQ);              // [kNQ] score part of the bound
   uint64_t* floor_key = reinterpret_cast<uint64_t*>(bnd_f + kNQ);      // [kNQ] pooled admission floor (see kPoolM)
   uint64_t* part_floor = floor_key + kNQ;                              // [4][kNQ] scratch of a floor refresh
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(part_floor + 4 * kNQ);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -81,36 +89,26 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
 #include "select_warps.inc.cuh"
 
   // ------------------------------------------------------------ one-time setup
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_corpus);
-    tma_prefetch_desc(&tm_q);
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&bar_full[s], 1);
-      mbar_init(&bar_empty[s], 1);
+      mbar_init(&bar_empty[s], 4);   // one arrive per warp of the wgmma warpgroup
     }
     for (int a = 0; a < kAccStages; ++a) {
-      mbar_init(&bar_tfull[a], 1);
+      mbar_init(&bar_tfull[a], 128); // every thread of the wgmma warpgroup, after its score stores
       mbar_init(&bar_tempty[a], 4);  // one arrive per select warp
     }
-    mbar_init(bar_q, 1);
     fence_mbar_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, kTmemCols);
-    tmem_relinquish();
   }
 #define CRAG_SELECT_SECTION 2
 #include "select_warps.inc.cuh"
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ================================================================ producer
-    if (elect_one()) {
-      mbar_arrive_expect_tx(bar_q, num_kb * kQBlockBytes);
-      for (int kb = 0; kb < num_kb; ++kb) tma_load_2d(&tm_q, bar_q, q_base + kb * kQBlockBytes, kb * kBlockK, 0);
+    if (lane == 0) {
+      tma_prefetch_desc(&tm_corpus);
+      tma_prefetch_desc(&tm_q);
       const uint64_t pol = policy_evict_first();
       int stage = 0;
       uint32_t phase = 0;
@@ -118,56 +116,71 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
         const int tile = tile_of(j);
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&bar_empty[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&bar_full[stage], kStageBytes);
+          mbar_arrive_expect_tx(&bar_full[stage], kStageTotalBytes);
           int tile_row0;
           if constexpr (IVF) tile_row0 = __ldg(&ivf.work[tile].x);
           else tile_row0 = tile * kTileRows;
-          tma_load_2d_hint(&tm_corpus, &bar_full[stage], stage_base + stage * kStageBytes, kb * kBlockK, tile_row0, pol);
+          uint8_t* st = stage_base + stage * kStageTotalBytes;
+          tma_load_2d_hint(&tm_corpus, &bar_full[stage], st, kb * kBlockK, tile_row0, pol);
+          tma_load_2d(&tm_q, &bar_full[stage], st + kStageBytes, kb * kBlockK, 0);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================================================== MMA issuer
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(kTileRows, kNQ);
-      mbar_wait(bar_q, 0);
-      tc_fence_after();
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&bar_tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * kNQ;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&bar_full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(stage_base + stage * kStageBytes);
-          const uint32_t b_addr = smem_u32(q_base + kb * kQBlockBytes);
+  } else if (warp >= kMmaWarp0) {
+    // ============================================================ wgmma warpgroup
+    // d[0]: rows 0-63 of the tile, d[1]: rows 64-127; this thread's rows 16 (warp % 4) + lane / 4 (+ 8) of each
+    const int frag_row = (warp - kMmaWarp0) * 16 + (lane >> 2);
+    const int frag_col = 2 * (lane & 3);
+    int stage = 0;
+    uint32_t phase = 0;
+    int acc = 0;
+    uint32_t acc_phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      float d[2][16];
 #pragma unroll
-          for (int ks = 0; ks < kBlockK / 16; ++ks) {
-            umma_f16(d_tmem, umma_desc_k_sw128(a_addr + ks * 32), umma_desc_k_sw128(b_addr + ks * 32), idesc,
-                     (kb | ks) != 0);
-          }
-          umma_commit(&bar_empty[stage]);  // smem slot reusable once these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      for (int i = 0; i < 16; ++i) d[0][i] = d[1][i] = 0.f;
+      int prev = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&bar_full[stage], phase);
+        const uint32_t a_addr = smem_u32(stage_base + stage * kStageTotalBytes);
+        const uint32_t b_addr = a_addr + kStageBytes;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kBlockK / 16; ++ks) {
+          const uint64_t db = wgmma_desc_sw128(b_addr + ks * 32);
+          wgmma_m64n32k16_ss(d[0], wgmma_desc_sw128(a_addr + ks * 32), db, 1u);
+          wgmma_m64n32k16_ss(d[1], wgmma_desc_sw128(a_addr + 64 * 128 + ks * 32), db, 1u);
         }
-        umma_commit(&bar_tfull[acc]);
-        if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+        wgmma_commit();
+        wgmma_wait<1>();   // k-block kb - 1 has retired: its smem slot goes back to the producer
+        if (kb > 0 && lane == 0) mbar_arrive(&bar_empty[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d[0]);
+      wgmma_fence_regs(d[1]);
+      if (lane == 0) mbar_arrive(&bar_empty[prev]);
+      mbar_wait(&bar_tempty[acc], acc_phase ^ 1);
+      float* st = score_tiles + acc * (kTileRows * kNQ);
+#pragma unroll
+      for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int j = 0; j < kNQ / 8; ++j)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int row = m * 64 + frag_row + (i >> 1) * 8;
+            st[score_slot(row, 8 * j + frag_col + (i & 1))] = d[m][4 * j + i];
+          }
+      mbar_arrive(&bar_tfull[acc]);
+      if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
     }
   } else {
     // ================================================================== select
 #define CRAG_SELECT_SECTION 3
 #include "select_warps.inc.cuh"
   }
-
-  // ------------------------------------------------------------------ teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // ------------------------------------------------------------------ host side
@@ -183,7 +196,7 @@ struct SearchPlan {
 SearchPlan plan_search(int k) {
   SearchPlan p;
   p.grid = sm_count();
-  if (p.grid <= 0) p.grid = 148;
+  if (p.grid <= 0) p.grid = 132;
   p.keys_bytes = ((size_t(p.grid) * kNQ * k * 8) + 255) & ~size_t(255);
   p.minmax_bytes = ((size_t(p.grid) * kNQ * 2 * 4) + 255) & ~size_t(255);
   p.pool_bytes = p.grid <= kPoolMaxCtas ? ((size_t(kNQ) * p.grid * kPoolSlots * 8 + 255) & ~size_t(255)) : 0;
@@ -210,7 +223,7 @@ int launch_search(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_r
                   int grid, const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift,
                   uint64_t* part_keys, float* part_minmax, cudaStream_t stream) {
   using L = SearchLayout<KLIST, CAP, STAGES>;
-  const size_t smem = L::smem_bytes(num_kb);
+  const size_t smem = L::smem_bytes();
   auto kern = search_topk_kernel<KLIST, CAP, STAGES>;
   int rc = ensure_smem_attr<KernelTag<KLIST, CAP, STAGES, false, false>>(kern, smem);
   if (rc != CRAG_OK) return rc;
@@ -224,7 +237,7 @@ template <int KLIST, int CAP, int STAGES>
 int launch_ivf_scan(const CUtensorMap& tm_res, const CUtensorMap& tm_q, int num_kb, int nq, int k, int grid,
                     uint64_t* pool, uint64_t* part_keys, float* part_minmax, const IvfArgs& ivf, cudaStream_t stream) {
   using L = SearchLayout<KLIST, CAP, STAGES>;
-  const size_t smem = L::smem_bytes(num_kb);
+  const size_t smem = L::smem_bytes();
   auto kern = search_topk_kernel<KLIST, CAP, STAGES, true>;
   int rc = ensure_smem_attr<KernelTag<KLIST, CAP, STAGES, true, false>>(kern, smem);
   if (rc != CRAG_OK) return rc;
@@ -293,8 +306,8 @@ int scan_pass(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_st
   if (!env_pool) pool = nullptr;
   const int shift = env_shift < 0 ? 0 : (env_shift > 6 ? 6 : env_shift);
   const uint32_t perm = env_shift < 0 ? 0u : perm_multiplier(num_tiles >> shift);
-  if (k <= 64) return launch_search<64, 64, 7>(tm_corpus, tm_q, int(n_rows), num_kb, nq, k, grid, after_keys, pool, perm, shift, part_keys, part_minmax, stream);
-  return launch_search<128, 128, 5>(tm_corpus, tm_q, int(n_rows), num_kb, nq, k, grid, after_keys, pool, perm, shift, part_keys, part_minmax, stream);
+  if (k <= 64) return launch_search<64, 64, 6>(tm_corpus, tm_q, int(n_rows), num_kb, nq, k, grid, after_keys, pool, perm, shift, part_keys, part_minmax, stream);
+  return launch_search<128, 128, 4>(tm_corpus, tm_q, int(n_rows), num_kb, nq, k, grid, after_keys, pool, perm, shift, part_keys, part_minmax, stream);
 }
 
 // merge the per-CTA partials of one pass into the final (ids, scores, minmax) of its <= 32 queries
@@ -386,8 +399,8 @@ extern "C" int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int
       pool = reinterpret_cast<uint64_t*>(ws + ip.pool_off);
       CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, sp.pool_bytes, stream));
     }
-    rc = (k <= 64) ? launch_ivf_scan<64, 64, 7>(tm_res, tm_q, num_kb, nqc, k, sp.grid, pool, part_keys, part_minmax, ivf, stream)
-                   : launch_ivf_scan<128, 128, 5>(tm_res, tm_q, num_kb, nqc, k, sp.grid, pool, part_keys, part_minmax, ivf, stream);
+    rc = (k <= 64) ? launch_ivf_scan<64, 64, 6>(tm_res, tm_q, num_kb, nqc, k, sp.grid, pool, part_keys, part_minmax, ivf, stream)
+                   : launch_ivf_scan<128, 128, 4>(tm_res, tm_q, num_kb, nqc, k, sp.grid, pool, part_keys, part_minmax, ivf, stream);
     if (rc != CRAG_OK) return rc;
     rc = finalize_parts(workspace, sp.grid, nqc, k, 0, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
                         out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, nullptr, sp, stream);
@@ -534,10 +547,10 @@ extern "C" int crag_search_scores(const void* corpus, int64_t n_rows, int dim, i
   rc = make_tmap_bf16_2d(&tm_corpus, corpus, uint64_t(n_rows), uint64_t(dim), uint64_t(corpus_row_stride) * 2, kTileRows);
   if (rc != CRAG_OK) return rc;
   const int num_kb = dim / kBlockK;
-  using L = SearchLayout<16, 16, 9>;
-  auto kern = search_topk_kernel<16, 16, 9, false, true>;
-  const size_t smem = L::smem_bytes(num_kb);
-  rc = ensure_smem_attr<KernelTag<16, 16, 9, false, true>>(kern, smem);
+  using L = SearchLayout<16, 16, 7>;
+  auto kern = search_topk_kernel<16, 16, 7, false, true>;
+  const size_t smem = L::smem_bytes();
+  rc = ensure_smem_attr<KernelTag<16, 16, 7, false, true>>(kern, smem);
   if (rc != CRAG_OK) return rc;
   for (int q0 = 0; q0 < nq; q0 += kNQ) {
     const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
@@ -604,10 +617,10 @@ extern "C" int crag_ivf_assign(const void* rows, int64_t n_rows, int dim, int64_
   rc = make_tmap_bf16_2d(&tm_rows, rows, uint64_t(n_rows), uint64_t(dim), uint64_t(row_stride) * 2, kTileRows);
   if (rc != CRAG_OK) return rc;
   const int num_kb = dim / kBlockK;
-  using L = SearchLayout<16, 16, 9>;
-  auto kern = search_topk_kernel<16, 16, 9, false, true>;
-  const size_t smem = L::smem_bytes(num_kb);
-  rc = ensure_smem_attr<KernelTag<16, 16, 9, false, true>>(kern, smem);
+  using L = SearchLayout<16, 16, 7>;
+  auto kern = search_topk_kernel<16, 16, 7, false, true>;
+  const size_t smem = L::smem_bytes();
+  rc = ensure_smem_attr<KernelTag<16, 16, 7, false, true>>(kern, smem);
   if (rc != CRAG_OK) return rc;
   // the pass over centroid block 0 initialises every row's running best (-inf, list 0); later passes update it
   for (int q0 = 0; q0 < nlist; q0 += kNQ) {

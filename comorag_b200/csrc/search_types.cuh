@@ -13,17 +13,31 @@ namespace crag {
 constexpr int kBlockK = 64;     // bf16 per 128-byte swizzle row
 constexpr int kStageBytes = kTileRows * kBlockK * 2;  // 16 KB
 constexpr int kQBlockBytes = kNQ * kBlockK * 2;       // 4 KB
-constexpr int kSearchThreads = 192;
+// One pipeline stage: a corpus box and the query block's slice of the same 64 columns.  Streaming the query slices
+// (L2 hits after the first tile) instead of keeping the whole [32, dim] block resident frees 64 KB at dim = 1024 for
+// stages and score tiles.
+constexpr int kStageTotalBytes = kStageBytes + kQBlockBytes;  // 20 KB
+// warps 0-3 select, warps 4-7 the wgmma warpgroup, warp 8 the TMA producer
+constexpr int kSearchThreads = 288;
 constexpr int kEpiThreads = 128;
-constexpr int kAccStages = 16;       // score-tile buffers in TMEM: the scan may run 16 tiles ahead of the select warps
-constexpr uint32_t kTmemCols = kAccStages * kNQ;  // 512 columns = all of TMEM (1 CTA per SM)
+constexpr int kMmaWarp0 = 4;
+constexpr int kProducerWarp = 8;
+// One score tile in shared memory: 128 rows x 32 fp32 scores, row r's score of query q at r * 32 + (q ^ (r % 32)) so
+// that a select warp reading one row per lane hits 32 distinct banks.  The wgmma warpgroup's stores of its accumulator
+// fragment (8 rows x 4 column pairs per warp instruction) still meet 4-way bank conflicts: 16 KB of stores per tile
+// against 256 KB of corpus reads at dim 1024, so the scan stays HBM-bound.
+constexpr int kScoreTileBytes = kTileRows * kNQ * 4;  // 16 KB
+__host__ __device__ constexpr int score_slot(int row, int q) { return row * kNQ + (q ^ (row & 31)); }
 
 template <int KLIST, int CAP, int STAGES>
 struct SearchLayout {
   static constexpr int kKeysPerQuery = KLIST + CAP;
+  // score-tile buffers: the scan may run this many tiles ahead of the select warps.  Together with STAGES they fill
+  // what the 227 KB of shared memory leave beside the candidate lists.
+  static constexpr int kAccStages = 4;
   __host__ __device__ static constexpr size_t keys_bytes() { return size_t(kNQ) * kKeysPerQuery * 8; }
   __host__ __device__ static constexpr size_t misc_bytes() {
-    return (2 * STAGES + 2 * kAccStages + 1) * 8    // mbarriers
+    return (2 * STAGES + 2 * kAccStages) * 8        // mbarriers
            + kNQ * 8               // thr_key
            + kNQ * 4               // thr_f
            + kNQ * 4               // cnt
@@ -31,10 +45,10 @@ struct SearchLayout {
            + kNQ * 8               // pooled admission floor (key)
            + 4 * kNQ * 8           // per-warp partial floors of a refresh
            + 4 * kNQ * 2 * 4       // min/max cross-warp reduction
-           + 16;                   // tmem base
+           + 16;
   }
-  __host__ static size_t smem_bytes(int num_kb) {
-    return 1024 + size_t(STAGES) * kStageBytes + size_t(num_kb) * kQBlockBytes + keys_bytes() + misc_bytes();
+  __host__ __device__ static constexpr size_t smem_bytes() {
+    return 1024 + size_t(STAGES) * kStageTotalBytes + size_t(kAccStages) * kScoreTileBytes + keys_bytes() + misc_bytes();
   }
 };
 
@@ -67,7 +81,7 @@ struct IvfArgs {
 struct NoIvfArgs {};
 // Score-all variant (SCORES = true): the full-array contracts of the reference -- get_fact_scores returns the score
 // of EVERY fact row (ComoRAG.py:937-948) and dense_passage_retrieval a permutation of ALL rows (:950-967, consumed
-// rank by rank by PPR at :1034-1042).  Same TMA -> tcgen05 -> TMEM stream; the select warps write the fp32 scores
+// rank by rank by PPR at :1034-1042).  Same TMA -> wgmma -> score-tile stream; the select warps write the fp32 scores
 // (out[q * ld + row], one coalesced 128-byte store per warp and query) instead of running the selector.
 struct ScoreArgs {
   float* out;

@@ -2,8 +2,8 @@
 // (CRAG_SELECT_SECTION = 1: the tile permutation, 2: the selector state's initialisation, 3: the whole select-warp
 // branch), so the kernel compiles from exactly the token stream it had when these lines stood in search.cu -- its
 // SASS is byte-identical -- while tests/warp_emu/select_emu_test.cpp includes the same three sections inside a host
-// function whose locals carry the same names (keys, thr_key, cnt, pool, k, nq, warp, lane, ...), maps tcgen05.ld to
-// a score matrix it supplies and the mbarrier / named-barrier operations to the fiber emulator, and so runs the
+// function whose locals carry the same names (keys, thr_key, cnt, pool, k, nq, warp, lane, ...), maps the score-tile
+// read (ld_score_row) to a score matrix it supplies and the mbarrier / named-barrier operations to the fiber emulator, and so runs the
 // selector of the headline kernel on the CPU: admission, warp-ballot compaction, flushes, pooled floor refreshes,
 // rank continuation, the score-all and IVF variants, the drain and the (min, max) reduction.
 // Not a header: it has no include guard and declares nothing at namespace scope.
@@ -31,8 +31,8 @@
     bnd_f[threadIdx.x] = (b == ~0ull) ? INFINITY : (b == 0ull ? -INFINITY : key_score(b));
   }
 #elif CRAG_SELECT_SECTION == 3
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may read
-    const int ew = warp - 2;    // select-warp index 0..3 (query ownership for flushes)
+    const int quad = warp;      // rows quad * 32 .. quad * 32 + 31 of every score tile
+    const int ew = warp;        // select-warp index 0..3 (query ownership for flushes)
     float mn[kNQ], mx[kNQ];
 #pragma unroll
     for (int q = 0; q < kNQ; ++q) { mn[q] = INFINITY; mx[q] = -INFINITY; }
@@ -121,11 +121,8 @@
         named_bar_sync(1, kEpiThreads);
       }
       mbar_wait(&bar_tfull[acc], acc_phase);
-      tc_fence_after();
       uint32_t r[kNQ];
-      tmem_ld_32x32b_x32(tmem_base + (uint32_t(quad * 32) << 16) + acc * kNQ, r);
-      tmem_ld_wait();
-      tc_fence_before();
+      ld_score_row(score_tiles + acc * (kTileRows * kNQ), quad * 32 + lane, r);
       __syncwarp();
       if (lane == 0) mbar_arrive(&bar_tempty[acc]);
       if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
@@ -174,7 +171,7 @@
         }
       } else {
         // this tile belongs to ONE coarse list: only the queries probing it see its rows, and a row's score is
-        // q . c_list (coarse pass, fp32) + q . residual (this tile's UMMA)
+        // q . c_list (coarse pass, fp32) + q . residual (this tile's wgmma)
         const int4 item = __ldg(&ivf.work[tile]);
         row = item.x + quad * 32 + lane;
         if (quad * 32 + lane < item.y) {

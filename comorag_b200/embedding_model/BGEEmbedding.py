@@ -1,4 +1,4 @@
-"""BGEEmbeddingModel call surface on the B200 engine (reference: embedding_model/BGEEmbedding.py).
+"""BGEEmbeddingModel call surface on the H100 engine (reference: embedding_model/BGEEmbedding.py).
 
 What is kept bit-for-bit from the reference's behaviour (SURVEY.md section 7 "reference quirks"):
   * `batch_encode` ALWAYS prefixes the passage instruction, whatever `instruction=` / `is_query=` say, and
@@ -8,7 +8,7 @@ What is kept bit-for-bit from the reference's behaviour (SURVEY.md section 7 "re
   * a bare `str` is treated as one text -> [1, D]; `norm=`, `num_workers=` ... kwargs are accepted and ignored;
   * `.encode(prompts, **kw)` is positional-friendly and returns a torch.Tensor [n, D] (BGEEmbedding.py:57-61),
     with NO instruction unless one is passed; `batch_encode` returns np.float32 [n, D] (C-contiguous).
-What differs: the forward runs on hand-written sm_100a kernels over an unpadded token stream with bf16
+What differs: the forward runs on hand-written sm_90a kernels over an unpadded token stream with bf16
 weights (see comorag_b200/encoder.py); batches are cut by a packed-token budget rather than only by
 `batch_size`, which changes nothing arithmetically because rows are independent.
 """

@@ -13,7 +13,7 @@ class OpenAIEmbeddingModel(BaseEmbeddingModel):
 
     def __init__(self, *args, **kwargs):
         raise NotImplementedError("OpenAIEmbeddingModel is an HTTP client in the reference and is out of scope "
-                                  "for the B200 engine; use a local 'bge-' checkpoint")
+                                  "for the H100 engine; use a local 'bge-' checkpoint")
 
 
 def _get_embedding_model_class(embedding_model_name: str = "None"):

@@ -1,4 +1,4 @@
-"""EmbeddingStore call surface on the B200 engine (reference: src/comorag/embedding_store.py).
+"""EmbeddingStore call surface on the H100 engine (reference: src/comorag/embedding_store.py).
 
 Same constructor, methods, attributes, return values, id scheme (namespace + "-" + md5(text),
 misc_utils.py:152-163) and parquet file (`vdb_<namespace>.parquet`, columns hash_id / content / embedding =
@@ -7,7 +7,7 @@ large_string / large_string / list<float>) as the reference, so ComoRAG.py and i
 What is different underneath:
   * rows live in one growing fp32 host matrix (not a Python list of N arrays) AND as bf16 rows of a
     device-resident DenseIndex, filled straight from the encoder's device output;
-  * `search(queries, k)` runs the fused sm_100a top-k kernel over the shard instead of callers pulling the
+  * `search(queries, k)` runs the fused sm_90a top-k kernel over the shard instead of callers pulling the
     whole matrix with get_embeddings() and doing np.dot + argsort per query (ComoRAG.py:937-967);
   * parquet I/O goes through pyarrow arrays built from the matrix (no per-row Python objects).
 """

@@ -111,7 +111,7 @@ class DenseIndex:
         self.dim = int(dim)
         self.dim_pad = _pad_dim(self.dim)
         if self.dim_pad > MAX_DIM:
-            raise ValueError(f"dim {dim} > {MAX_DIM} is not supported by the sm_100a search kernel")
+            raise ValueError(f"dim {dim} > {MAX_DIM} is not supported by the sm_90a search kernel")
         if device is None:
             if not torch.cuda.is_available():
                 raise _native.NativeError("DenseIndex needs a CUDA device (no CPU fallback)")

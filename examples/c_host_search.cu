@@ -123,7 +123,7 @@ static CaseResult run_case(int64_t rows, int dim, int nq, int k, int reps, uint1
   cudaStream_t st;
   CUDA_OK(cudaStreamCreate(&st));
   const size_t n_elems = (size_t)rows * dim;
-  fill_rows<<<148 * 8, 256, 0, st>>>(d_rows, n_elems, sqrtf(3.0f / dim), 0xC0FFEEull + (uint64_t)rows);
+  fill_rows<<<132 * 8, 256, 0, st>>>(d_rows, n_elems, sqrtf(3.0f / dim), 0xC0FFEEull + (uint64_t)rows);
   CUDA_OK(cudaGetLastError());
 
   // queries: random unit vectors, rounded to bf16; planted rows from the ROUNDED query values

@@ -1,5 +1,5 @@
 /*
- * libcomorag_b200 -- C ABI of the B200 (sm_100a) embedding + dense-retrieval
+ * libcomorag_b200 -- C ABI of the H100 (sm_90a) embedding + dense-retrieval
  * engine that sits behind ComoRAG's embedding_model / EmbeddingStore call
  * surfaces.
  *
@@ -49,7 +49,7 @@ typedef void* crag_stream_t;
 CRAG_API int crag_version(void);
 /* Message for the last failing call made by the calling thread ("" if none). */
 CRAG_API const char* crag_last_error(void);
-/* Number of SMs of the current device (148 on B200); <0 on error. */
+/* Number of SMs of the current device (132 on H100 SXM); <0 on error. */
 CRAG_API int crag_sm_count(void);
 
 /* Growable device buffer for a corpus shard that is appended to (EmbeddingStore.insert_strings, embedding_store.py:63-90):
@@ -160,7 +160,7 @@ CRAG_API int crag_search_finalize_exchange(const void* workspace, size_t workspa
  *     query_fact_scores = np.dot(self.fact_embeddings, q.T)            (ComoRAG.py:944; get_fact_scores returns all
  *                                                                      N_f scores and callers index them, :475,:1054)
  *     query_doc_scores  = np.dot(self.passage_embeddings, q.T)         (ComoRAG.py:958-960)
- * The same TMA -> tcgen05 stream as crag_search_topk, but the select warps store the fp32 scores instead of
+ * The same TMA -> wgmma stream as crag_search_topk, but the select warps store the fp32 scores instead of
  * running the top-k selector.  out_scores device fp32, query q's row r at out_scores[q * out_ld + r]
  * (out_ld >= n_rows); out_minmax device fp32 [nq, 2] or NULL.  Other arguments and the workspace as
  * crag_search_topk (crag_search_workspace_bytes(nq, 1) bytes suffice). */
@@ -191,7 +191,7 @@ CRAG_API int crag_rank_scores(const float* scores, int64_t n, int64_t* out_ids, 
  *   residual  device bf16 [m, n] (ldr), only for CRAG_GEMM_BIAS_RESIDUAL
  *   out       device bf16 [m, n] (ldo)
  * n, k, and all leading dimensions must be multiples of 8; pointers 16-B aligned.
- * Accumulation is fp32 on the tcgen05 tensor cores.
+ * Accumulation is fp32 on the wgmma tensor cores.
  */
 #define CRAG_GEMM_BIAS 0          /* out = acc + bias */
 #define CRAG_GEMM_BIAS_GELU 1     /* out = gelu_erf(acc + bias) */
@@ -210,7 +210,7 @@ CRAG_API int crag_gemm_bf16(const void* a, int64_t lda, const void* w, int64_t l
  * The caller runs the coarse pass itself (crag_search_topk over the bf16 centroid table with k = nprobe) and
  * passes its output: probed_ids int64 [nq, nprobe] (-1 = absent), probed_scores fp32 [nq, nprobe] = q . c_list.
  * Per block of 32 queries: a plan kernel marks which queries probe which list and compacts the probed lists'
- * tiles into a work-list; the scan kernel (the flat kernel's TMA/tcgen05/selector pipeline walking that work-list)
+ * tiles into a work-list; the scan kernel (the flat kernel's TMA/wgmma/selector pipeline walking that work-list)
  * scores  q . c_list + q . residual  for the probing queries only; the per-CTA lists are merged and stored-row ids
  * mapped to original ids.  Outputs as crag_search_topk (min/max range over the probed rows).
  * workspace >= crag_ivf_workspace_bytes(nlist, total_tiles, k), 256-byte aligned. */
@@ -324,8 +324,8 @@ CRAG_API int crag_pool_normalize(const void* hidden, const int32_t* cu_seqlens, 
 CRAG_API int crag_attention_varlen(const void* qkv, const int32_t* cu_seqlens, int n_seqs, int max_seqlen,
                                    int hidden_size, int heads, void* ctx, crag_stream_t stream);
 
-/* The same attention on the tcgen05 tensor cores (head dim 64 only): S = Q K^T and O += P V as UMMA tiles with TMEM
- * accumulators, Q/K/V staged by TMA.  total_tokens = rows of qkv (sizes the TMA tensor map). */
+/* The same attention on the wgmma tensor cores (head dim 64 only): S = Q K^T and O += P V as wgmma tiles with
+ * register accumulators, Q/K/V staged by TMA.  total_tokens = rows of qkv (sizes the TMA tensor map). */
 CRAG_API int crag_attention_varlen_tc(const void* qkv, const int32_t* cu_seqlens, int n_seqs, int total_tokens,
                                       int max_seqlen, int hidden_size, int heads, void* ctx, crag_stream_t stream);
 

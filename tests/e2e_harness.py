@@ -9,8 +9,8 @@
 
 The same harness drives both arms -- the reference's own classes on CPU and the comorag_b200 shim on cuda:0 -- so
 whatever the stand-ins approximate, they approximate identically for both.  Nothing in here is product code; nothing
-in comorag_b200/ imports it.  The reference tree is looked up at $COMORAG_REFERENCE, /root/reference (build container)
-or <repo>/baseline/_ref (an unmodified copy staged by tools/stage_reference.sh, git-ignored, travels to the GPU box).
+in comorag_b200/ imports it.  The reference tree is looked up at $COMORAG_REFERENCE, then at <repo>/oracle/_ref (the
+unmodified copy build() stages there, oracle/stage_reference.py).
 """
 from __future__ import annotations
 
@@ -30,7 +30,7 @@ CKPT = os.path.join(ROOT, "tests", "golden", "bge-tiny-synth")
 
 
 def find_reference_root() -> Optional[str]:
-    for cand in (os.environ.get("COMORAG_REFERENCE"), "/root/reference", os.path.join(ROOT, "baseline", "_ref")):
+    for cand in (os.environ.get("COMORAG_REFERENCE"), os.path.join(ROOT, "oracle", "_ref")):
         if cand and os.path.isdir(os.path.join(cand, "src", "comorag")) and \
                 os.path.isdir(os.path.join(cand, "dataset", "cinderella")):
             return cand

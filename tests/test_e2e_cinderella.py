@@ -3,8 +3,8 @@ config 1; entry point main_openai.py:23-25), driven offline by tests/e2e_harness
 stand-ins), once on the reference's own classes (CPU, fp32 HF encoder + numpy search) and once on the comorag_b200 shim
 (cuda:0) -- then the retrieved ids / scores of every question and probe are compared.
 
-The reference tree is not in this repository: the tests use /root/reference in the build container and the unmodified
-copy staged under baseline/_ref (tools/stage_reference.sh) on the GPU box, and skip when neither exists.
+The reference tree is not in this repository: the tests use the unmodified copy build() stages under oracle/_ref
+(oracle/stage_reference.py) or the checkout $COMORAG_REFERENCE names, and skip when neither exists.
 """
 import json
 import os
@@ -20,7 +20,7 @@ import e2e_harness as H  # noqa: E402
 
 GOLDEN = os.path.join(HERE, "golden", "e2e_cinderella_reference.json")
 REF_ROOT = H.find_reference_root()
-needs_ref = pytest.mark.skipif(REF_ROOT is None, reason="reference tree not present (run tools/stage_reference.sh)")
+needs_ref = pytest.mark.skipif(REF_ROOT is None, reason="reference tree not present (build() stages it under oracle/_ref)")
 
 _cache = {}
 

@@ -56,7 +56,7 @@ def test_gemm_epilogues(dev, M, N, K, epi):
                                              (768, 12, [128] * 3, 0), (128, 2, [5, 64, 65, 1, 130, 128, 129, 300, 512], 1),
                                              (1024, 16, [512, 33, 200, 511], 1), (768, 12, [128, 63, 64], 1)])
 def test_varlen_attention(dev, H, heads, lens, tc):
-    """tc=0: mma.sync kernel (any head dim in {32, 64}); tc=1: tcgen05 kernel (head dim 64)."""
+    """tc=0: mma.sync kernel (any head dim in {32, 64}); tc=1: wgmma kernel (head dim 64)."""
     from comorag_b200 import _native
     lib = _native.load()
     dh, T = H // heads, sum(lens)

@@ -1,5 +1,5 @@
 """The SIMT parts of the kernels on the CPU.  csrc/topk.cuh, pool_floor.cuh, merge_kernels.cuh, rank_kernels.cuh and
-encoder_simt.cuh hold no tcgen05 / TMA / mbarrier code, so the SAME headers the library compiles are compiled for the
+encoder_simt.cuh hold no wgmma / TMA / mbarrier code, so the SAME headers the library compiles are compiled for the
 host with CUDA threads as fibers (tests/warp_emu: warp collectives, __syncthreads, shared memory, one OS thread per
 rank with real atomics for the cross-rank exchange) and checked against plain C++ models:
   selector_emu_test.cpp  bitonic sort, flush / insert list maintenance, select_stream, and the pooled admission
@@ -7,7 +7,7 @@ rank with real atomics for the cross-rank exchange) and checked against plain C+
   select_emu_test.cpp    the SELECT WARPS of the headline kernel (csrc/select_warps.inc.cuh, the text search_topk_kernel
                          #includes): admission, warp-ballot compaction, flushes, pooled-floor refreshes across CTAs,
                          drain, rank continuation, score-all and IVF variants -- fed a score matrix in place of
-                         tcgen05.ld, merged by the emulated merge kernel, compared bit for bit with the exact top-k
+                         the score-tile read, merged by the emulated merge kernel, compared bit for bit with the exact top-k
   encoder_emu_test.cpp   embedding + LayerNorm, LayerNorm, masked mean pool + L2 normalise (K3) and the classifier
                          head (csrc/encoder_simt.cuh) against double-precision models
   kernel_emu_test.cpp    the IVF plan / id-map kernels, the radix-rank kernels (full permutation == stable descending

@@ -319,8 +319,10 @@ def test_headline_shape_10m_rows_ids_exact(dev, k):
     want_i, want_s, want_mm, gaps = torch_reference_topk(corpus, queries, k)
     so.assert_topk_matches(ids.cpu().numpy(), scores.double().cpu().numpy(), want_i, want_s, gaps, score_tol=1e-3)
     np.testing.assert_allclose(mm.cpu().numpy(), want_mm, atol=1e-5)
-    # 20.48 GB per pass: anything slower than 4 ms (5.1 TB/s) means the selector, not HBM, set the pace
-    assert ms < 4.0, f"10M x 1024 top-{k} pass took {ms:.2f} ms"
+    # 20.48 GB per pass take 6.11 ms at the H100's data-sheet 3.35 TB/s: a pass more than 30 % above that floor
+    # (7.95 ms, 2.58 TB/s) means the selector, not HBM, set the pace
+    hbm_floor_ms = n * dim * 2 / 3.35e12 * 1e3
+    assert ms < 1.3 * hbm_floor_ms, f"10M x 1024 top-{k} pass took {ms:.2f} ms (HBM floor {hbm_floor_ms:.2f} ms)"
 
 
 def _adversarial_corpus(kind, n, dim, queries, dev):

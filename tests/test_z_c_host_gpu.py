@@ -10,8 +10,7 @@ import pytest
 @pytest.mark.gpu
 def test_c_host_search_ids_exact_through_the_c_abi():
     """crag_search_topk called from a plain CUDA-runtime host: planted-neighbour shards whose exact top-k is known in
-    closed form (ids exact, scores / max within 1e-3).  Shapes = one rank's shard of the 8-GPU split, the cases of
-    profiles/r02_c_host_search_final.jsonl."""
+    closed form (ids exact, scores / max within 1e-3).  Shapes = one rank's shard of the 8-GPU split."""
     from comorag_b200 import build
     exe = build.build_examples()
     for rows, dim, nq, k in ((1_250_000, 1024, 32, 10), (1_250_000, 1024, 32, 100), (1_250_000, 1024, 32, 128)):

@@ -6,11 +6,16 @@ import torch
 
 
 def make_unit_rows(n: int, dim: int, seed: int, device="cpu") -> torch.Tensor:
-    """Seeded N(0,1) rows, L2-normalised in fp32, rounded to bf16 (SURVEY.md 8d synthetic corpus)."""
+    """Seeded N(0,1) rows, L2-normalised in fp32, rounded to bf16 (SURVEY.md 8d synthetic corpus).  Generated in
+    slabs of at most 2^28 fp32 values (1 GiB), so that a 10M x 1024 corpus fits on an 80 GB GPU; below one slab the
+    rows are those of a single randn call."""
     g = torch.Generator(device=device).manual_seed(seed)
-    x = torch.randn((n, dim), generator=g, device=device, dtype=torch.float32)
-    x = torch.nn.functional.normalize(x, dim=1)
-    return x.to(torch.bfloat16)
+    out = torch.empty((n, dim), dtype=torch.bfloat16, device=device)
+    slab = max(1, (1 << 28) // dim)
+    for s0 in range(0, n, slab):
+        x = torch.randn((min(slab, n - s0), dim), generator=g, device=device, dtype=torch.float32)
+        out[s0:s0 + x.shape[0]] = torch.nn.functional.normalize(x, dim=1).to(torch.bfloat16)
+    return out
 
 
 def torch_reference_topk(corpus_bf16: torch.Tensor, queries_bf16: torch.Tensor, k: int, row_offset: int = 0,

@@ -1,7 +1,7 @@
 // The select warps of the shard-scan kernel on the CPU.  csrc/select_warps.inc.cuh is the TEXT of search_topk_kernel's
 // select-warp code (the kernel #includes it, its SASS is unchanged); here the same three sections are included inside
 // a host function whose locals carry the names the kernel's have, with
-//   tcgen05.ld            -> a score matrix this test supplies (the selection logic does not care where scores come
+//   score-tile read       -> a score matrix this test supplies (the selection logic does not care where scores come
 //                            from: any fp32 matrix is a valid "q . x" for it, ties and adversarial orders included)
 //   mbarrier waits        -> nothing (a tile is "there" when it is asked for)
 //   named barriers        -> the fiber emulator's (warp_emu.h)

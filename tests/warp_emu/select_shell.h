@@ -1,6 +1,6 @@
 // search_topk_kernel's select warps inside a host function (see select_emu_test.cpp): csrc/select_warps.inc.cuh is the
-// text the kernel #includes; here the same three sections are included with tcgen05.ld mapped to a score matrix the
-// caller supplies, mbarrier waits to nothing and the named barriers to the fiber emulator.
+// text the kernel #includes; here the same three sections are included with the score-tile read mapped to a score
+// matrix the caller supplies, mbarrier waits to nothing and the named barriers to the fiber emulator.
 #pragma once
 #include <cuda_runtime.h>   // the stub
 
@@ -13,31 +13,28 @@ namespace crag {
 // ---- host stand-ins for the ptx.cuh operations the select warps use
 static inline void mbar_wait(uint64_t*, uint32_t) {}
 static inline void mbar_arrive(uint64_t*) {}
-static inline void tc_fence_after() {}
-static inline void tc_fence_before() {}
-static inline void tmem_ld_wait() {}
 static inline void named_bar_sync(uint32_t id, uint32_t n) { warp_emu::named_barrier(int(id), int(n)); }
 static inline bool named_bar_or(uint32_t id, uint32_t n, bool p) { return warp_emu::named_barrier_or(int(id), int(n), p); }
 
-// the score tiles "in TMEM": scores[row * kNQ + q]; rows past the end read as 0 (TMA zero-fills out-of-bounds boxes)
+// the score tiles: scores[row * kNQ + q]; rows past the end read as 0 (TMA zero-fills out-of-bounds boxes)
 struct ScoreSource {
   const float* scores = nullptr;
   int64_t rows = 0;
   const int4* work = nullptr;      // IVF: the tile index is a work-list index, the rows are work[tile].x + ...
 };
 static thread_local ScoreSource g_src;
-static inline void emu_tmem_ld(int tile, int quad, int lane, uint32_t (&r)[32]) {
+static inline void emu_score_ld(int tile, int quad, int lane, uint32_t (&r)[32]) {
   const int64_t row = (g_src.work ? int64_t(g_src.work[tile].x) : int64_t(tile) * kTileRows) + quad * 32 + lane;
   for (int q = 0; q < kNQ; ++q) r[q] = row < g_src.rows ? __float_as_uint(g_src.scores[row * kNQ + q]) : 0u;
 }
-// the kernel's call is tmem_ld_32x32b_x32(<TMEM address>, r); `tile`, `quad`, `lane` are locals of the included text
-#define tmem_ld_32x32b_x32(addr, r) emu_tmem_ld(tile, quad, lane, r)
+// the kernel's call is ld_score_row(<score tile>, <row in tile>, r); `tile`, `quad`, `lane` are locals of the included text
+#define ld_score_row(buf, row_in_tile, r) emu_score_ld(tile, quad, lane, r)
 
 // search_topk_kernel without its producer / MMA warps: same parameter names, same local names.  Launch with
 // select_shell_smem_bytes<KLIST, CAP>() of dynamic shared memory.
 template <int KLIST, int CAP>
 constexpr size_t select_shell_smem_bytes() {
-  return size_t(kNQ) * (KLIST + CAP) * 8 + 2 * kAccStages * 8 + kNQ * (8 + 4 + 4) + 4 * kNQ * 2 * 4 + kNQ * (8 + 4 + 8) + 4 * kNQ * 8 + 64;
+  return size_t(kNQ) * (KLIST + CAP) * 8 + 2 * SearchLayout<KLIST, CAP, 1>::kAccStages * 8 + kNQ * (8 + 4 + 4) + 4 * kNQ * 2 * 4 + kNQ * (8 + 4 + 8) + 4 * kNQ * 8 + 64;
 }
 
 template <int KLIST, int CAP, int STAGES, bool IVF = false, bool SCORES = false>
@@ -45,6 +42,7 @@ static void search_select_shell(int n_rows, int nq, int k, const uint64_t* after
                                 int perm_shift, uint64_t* part_keys, float* part_minmax,
                                 const typename IvfParam<IVF, SCORES>::type ivf) {
   using L = SearchLayout<KLIST, CAP, STAGES>;
+  constexpr int kAccStages = L::kAccStages;
   // the selector state, carved out of the block's dynamic shared memory as the kernel carves it out of smem_raw
   uint8_t* smem = static_cast<uint8_t*>(warp_emu::dynamic_shared());
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem);
@@ -68,9 +66,9 @@ static void search_select_shell(int n_rows, int nq, int k, const uint64_t* after
 #define CRAG_SELECT_SECTION 2
 #include "select_warps.inc.cuh"
   __syncthreads();
-  const uint32_t tmem_base = 0;
-  (void)tmem_base; (void)bar_tfull; (void)bar_tempty;
-  if (warp < 2) return;            // the TMA producer and the MMA issuer: nothing to emulate
+  const float* score_tiles = nullptr;
+  (void)score_tiles; (void)bar_tfull; (void)bar_tempty;
+  if (warp >= kMmaWarp0) return;   // the wgmma warpgroup and the TMA producer: nothing to emulate
   {
 #define CRAG_SELECT_SECTION 3
 #include "select_warps.inc.cuh"

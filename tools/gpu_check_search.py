@@ -1,4 +1,4 @@
-"""First-light / regression check of the search kernel on a real B200.
+"""First-light / regression check of the search kernel on a real H100.
 
 Each case runs in its own subprocess with a timeout, so a trap or hang in one
 case cannot take the others (or the box) down.  Usage (on the GPU box):
