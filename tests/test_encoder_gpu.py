@@ -1,7 +1,6 @@
 """GPU parity of the encoder path: each kernel against a plain torch fp32 statement of the same op, the whole forward
 against the torch oracle, and the drop-in BGEEmbeddingModel / EmbeddingStore against embeddings the REFERENCE produced
 for the synthetic checkpoint (tests/golden/encoder_golden.npz)."""
-import math
 import os
 
 import numpy as np
@@ -28,59 +27,9 @@ def gold():
     return np.load(os.path.join(HERE, "golden", "encoder_golden.npz"), allow_pickle=True)
 
 
-@pytest.mark.parametrize("M,N,K,epi", [(128, 128, 64, 0), (300, 384, 384, 0), (1000, 1152, 384, 0), (777, 1536, 384, 1),
-                                       (512, 384, 1536, 2), (2048, 3072, 1024, 0), (2048, 1024, 4096, 2), (2048, 4096, 1024, 1),
-                                       (1, 768, 768, 0), (129, 8, 8, 0)])
-def test_gemm_epilogues(dev, M, N, K, epi):
-    from comorag_b200 import _native
-    lib = _native.load()
-    g = torch.Generator(device=dev).manual_seed(M + N + K)
-    a = (torch.randn(M, K, generator=g, device=dev) * 0.5).bfloat16()
-    w = (torch.randn(N, K, generator=g, device=dev) * 0.05).bfloat16()
-    bias = torch.randn(N, generator=g, device=dev)
-    res = torch.randn(M, N, generator=g, device=dev).bfloat16()
-    out = torch.full((M, N), float("nan"), dtype=torch.bfloat16, device=dev)
-    rc = lib.crag_gemm_bf16(a.data_ptr(), K, w.data_ptr(), K, bias.data_ptr(), res.data_ptr(), N, out.data_ptr(), N, M, N, K,
-                            epi, torch.cuda.current_stream().cuda_stream)
-    _native.check(rc, "crag_gemm_bf16")
-    ref = a.float() @ w.float().T + bias
-    if epi == 1:
-        ref = torch.nn.functional.gelu(ref)
-    if epi == 2:
-        ref = ref + res.float()
-    err = (out.float() - ref).abs()
-    assert bool((err <= 0.01 * ref.abs() + 0.02).all()), float(err.max())   # bf16 output rounding
-
-
-@pytest.mark.parametrize("H,heads,lens,tc", [(128, 4, [5, 64, 65, 1, 130], 0), (1024, 16, [512, 33, 200], 0), (384, 12, [77, 512], 0),
-                                             (768, 12, [128] * 3, 0), (128, 2, [5, 64, 65, 1, 130, 128, 129, 300, 512], 1),
-                                             (1024, 16, [512, 33, 200, 511], 1), (768, 12, [128, 63, 64], 1)])
-def test_varlen_attention(dev, H, heads, lens, tc):
-    """tc=0: mma.sync kernel (any head dim in {32, 64}); tc=1: wgmma kernel (head dim 64)."""
-    from comorag_b200 import _native
-    lib = _native.load()
-    dh, T = H // heads, sum(lens)
-    g = torch.Generator(device=dev).manual_seed(H)
-    qkv = torch.randn(T, 3 * H, generator=g, device=dev).bfloat16()
-    cu = torch.tensor([0] + np.cumsum(lens).tolist(), dtype=torch.int32, device=dev)
-    ctx = torch.full((T, H), float("nan"), dtype=torch.bfloat16, device=dev)
-    st = torch.cuda.current_stream().cuda_stream
-    if tc:
-        rc = lib.crag_attention_varlen_tc(qkv.data_ptr(), cu.data_ptr(), len(lens), T, max(lens), H, heads, ctx.data_ptr(), st)
-    else:
-        rc = lib.crag_attention_varlen(qkv.data_ptr(), cu.data_ptr(), len(lens), max(lens), H, heads, ctx.data_ptr(), st)
-    _native.check(rc, "crag_attention_varlen")
-    ref, s = torch.zeros(T, H, device=dev), 0
-    for L in lens:
-        x = qkv[s:s + L].float()
-        q, k, v = (x[:, j * H:(j + 1) * H].view(L, heads, dh).transpose(0, 1) for j in range(3))
-        ref[s:s + L] = (torch.softmax(q @ k.transpose(-1, -2) / math.sqrt(dh), -1) @ v).transpose(0, 1).reshape(L, H)
-        s += L
-    assert float((ctx.float() - ref).abs().max()) < 0.03
-
-
 @pytest.mark.parametrize("H", [128, 384, 768, 1024])
 def test_layernorm(dev, H):
+    """Within one bf16 step of a float64 LayerNorm, the bound encoder_emu_test.cpp holds the same kernel to."""
     from comorag_b200 import _native
     lib = _native.load()
     g = torch.Generator(device=dev).manual_seed(H)
@@ -89,8 +38,9 @@ def test_layernorm(dev, H):
     out = torch.zeros_like(x)
     _native.check(lib.crag_layernorm(x.data_ptr(), 1001, H, gam.data_ptr(), bet.data_ptr(), 1e-12, out.data_ptr(),
                                      torch.cuda.current_stream().cuda_stream), "crag_layernorm")
-    ref = torch.nn.functional.layer_norm(x.float(), (H,), gam, bet, 1e-12)
-    assert bool(((out.float() - ref).abs() <= 0.01 * ref.abs() + 0.01).all())
+    ref = torch.nn.functional.layer_norm(x.double(), (H,), gam.double(), bet.double(), 1e-12)
+    step = ref.abs().clamp(min=1e-3) * 2.0 ** -7
+    assert bool(((out.double() - ref).abs() <= step).all()), float(((out.double() - ref).abs() / step).max())
 
 
 def test_pool_normalize_matches_reference_pooling(dev):
