@@ -70,6 +70,9 @@ SIGNATURES = {
                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "crag_rank_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "crag_rank_scores": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "crag_knn_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "crag_knn_topk": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_int,
+                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "crag_merge_topk": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_void_p]),
 }

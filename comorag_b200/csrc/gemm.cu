@@ -12,6 +12,8 @@
 //   warp 8     TMA producer: A box 128x64, W box 128x64 (128-byte swizzle)
 //              through a STAGES-deep mbarrier ring
 // With two CTAs resident, one CTA's epilogue overlaps the other's main loop.
+// A fourth, internal epilogue (GEMM_EPI_SCORES_F32, gemm_scores_f32) stores the raw fp32 accumulators: the score
+// block Q . X^T of crag_knn_topk (search.cu), on a 1-D grid with the query blocks fastest.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -74,7 +76,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n_blk = blockIdx.x, m_blk = blockIdx.y;
+  int n_blk = blockIdx.x, m_blk = blockIdx.y;
+  if constexpr (EPI == GEMM_EPI_SCORES_F32) {
+    // 1-D grid with the query blocks fastest: the CTAs in flight share a few corpus tiles and the chunk's queries
+    // stay in L2, so the corpus is read from HBM once per chunk (and N may exceed gridDim.y's 65535 tiles)
+    const int m_blocks = (M + kGemmBM - 1) / kGemmBM;
+    m_blk = int(blockIdx.x % unsigned(m_blocks));
+    n_blk = int(blockIdx.x / unsigned(m_blocks));
+  }
   const int num_kb = (K + kGemmBK - 1) / kGemmBK;
 
   if (threadIdx.x == 0) {
@@ -130,6 +139,27 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
   wgmma_wait<0>();
   wgmma_fence_regs(acc);
 
+  if constexpr (EPI == GEMM_EPI_SCORES_F32) {
+    // fp32 scores straight from the accumulator fragment, no bias; `out` carries the fp32 block.  N may be odd, so
+    // each element of a pair is guarded on its own
+    float* outf = reinterpret_cast<float*>(out);
+    const int srow0 = m_blk * kGemmBM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int scol0 = n_blk * kGemmBN + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < kGemmBN / 8; ++j) {
+      const int col = scol0 + 8 * j;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = srow0 + 8 * h;
+        if (row >= M) continue;
+        float* p = outf + int64_t(row) * ldo + col;
+        if (col + 1 < N) *reinterpret_cast<float2*>(p) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        else if (col < N) p[0] = acc[4 * j + 2 * h];
+      }
+    }
+    return;
+  }
+
   // epilogue: bias (+GELU | +residual), bf16 pairs straight from the accumulator fragment
   const int row0 = m_blk * kGemmBM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const int col0 = n_blk * kGemmBN + 2 * (lane & 3);
@@ -171,7 +201,8 @@ static int launch_gemm_t(const CUtensorMap& tm_a, const CUtensorMap& tm_b, int M
       if (dev >= 0 && dev < 64) done[dev] = true;
     }
   }
-  const dim3 grid((N + kGemmBN - 1) / kGemmBN, (M + kGemmBM - 1) / kGemmBM);
+  const unsigned n_blocks = (N + kGemmBN - 1) / kGemmBN, m_blocks = (M + kGemmBM - 1) / kGemmBM;
+  const dim3 grid = EPI == GEMM_EPI_SCORES_F32 ? dim3(m_blocks * n_blocks) : dim3(n_blocks, m_blocks);
   kern<<<grid, kGemmThreads, GemmLayout::smem_bytes(), stream>>>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
@@ -198,6 +229,21 @@ int gemm_bf16(const void* a, int64_t lda, const void* w, int64_t ldw, const floa
     case GEMM_EPI_BIAS_RESIDUAL: return launch_gemm_t<GEMM_EPI_BIAS_RESIDUAL>(tm_a, tm_b, M, N, K, bias, res, ldr, o, ldo, stream);
   }
   return fail(CRAG_ERR_INVALID, "gemm: unknown epilogue %d", epi);
+}
+
+int gemm_scores_f32(const void* a, int64_t lda, const void* w, int64_t ldw, float* out, int64_t ldo, int M, int N,
+                    int K, cudaStream_t stream) {
+  if (M <= 0 || N <= 0) return CRAG_OK;
+  if (K < 64 || K % 64 != 0 || lda % 8 || ldw % 8 || ldo % 2) return fail(CRAG_ERR_INVALID, "gemm scores: K must be a multiple of 64, lda/ldw multiples of 8 and ldo even");
+  if ((uintptr_t(a) | uintptr_t(w)) & 15 || uintptr_t(out) & 7) return fail(CRAG_ERR_INVALID, "gemm scores: misaligned pointer");
+  if (int64_t((M + kGemmBM - 1) / kGemmBM) * ((N + kGemmBN - 1) / kGemmBN) > int64_t(0x7FFFFFFF)) return fail(CRAG_ERR_INVALID, "gemm scores: too many tiles (M=%d N=%d)", M, N);
+  CUtensorMap tm_a, tm_b;
+  int rc = make_tmap_bf16_2d(&tm_a, a, uint64_t(M), uint64_t(K), uint64_t(lda) * 2, kGemmBM);
+  if (rc != CRAG_OK) return rc;
+  rc = make_tmap_bf16_2d(&tm_b, w, uint64_t(N), uint64_t(K), uint64_t(ldw) * 2, kGemmBN);
+  if (rc != CRAG_OK) return rc;
+  return launch_gemm_t<GEMM_EPI_SCORES_F32>(tm_a, tm_b, M, N, K, nullptr, nullptr, 0, reinterpret_cast<__nv_bfloat16*>(out),
+                                            ldo, stream);
 }
 
 }  // namespace crag

@@ -29,7 +29,9 @@
 // keeps each row's running argmax over centroid blocks (crag_ivf_assign).
 // Around it in this file: the per-shard merge (merge_topk_kernel), the fused
 // finalize + NVLink exchange + global merge of the row-sharded index
-// (finalize_exchange_kernel), and the C-ABI entry points.
+// (finalize_exchange_kernel), the C-ABI entry points, and crag_knn_topk -- exact
+// top-k up to k = 2048 for large query batches as a score-block GEMM (gemm.cu)
+// plus a per-query radix select (knn_select.cuh).
 #include "common.cuh"
 #include "ptx.cuh"
 #include "topk.cuh"
@@ -37,6 +39,8 @@
 #include "merge_kernels.cuh"
 #include "ivf_kernels.cuh"
 #include "search_types.cuh"
+#include "gemm.cuh"
+#include "knn_select.cuh"
 
 namespace crag {
 
@@ -262,8 +266,9 @@ namespace crag {
 namespace {
 
 int check_search_args(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride, const void* queries,
-                      int nq, int k, const void* workspace, size_t workspace_bytes, const SearchPlan& plan) {
-  if (nq < 1 || k < 1 || k > 128) return fail(CRAG_ERR_INVALID, "search: need nq >= 1 and 1 <= k <= 128 (nq=%d k=%d)", nq, k);
+                      int nq, int k, const void* workspace, size_t workspace_bytes, const SearchPlan& plan,
+                      int k_max = 128) {
+  if (nq < 1 || k < 1 || k > k_max) return fail(CRAG_ERR_INVALID, "search: need nq >= 1 and 1 <= k <= %d (nq=%d k=%d)", k_max, nq, k);
   if (dim < 64 || dim > 1024 || dim % 64 != 0) return fail(CRAG_ERR_INVALID, "search: dim must be a multiple of 64 in [64, 1024] (dim=%d)", dim);
   if (n_rows < 0 || n_rows >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "search: n_rows out of range (%lld)", (long long)n_rows);
   if (corpus_row_stride < dim || corpus_row_stride % 8 != 0) return fail(CRAG_ERR_INVALID, "search: corpus_row_stride must be >= dim and a multiple of 8");
@@ -460,6 +465,48 @@ extern "C" int crag_search_topk(const void* corpus, int64_t n_rows, int dim, int
                                 crag_stream_t stream) {
   return crag_search_topk_after(corpus, n_rows, dim, corpus_row_stride, row_offset, queries, nq, k, nullptr, out_ids,
                                 out_scores, out_minmax, nullptr, workspace, workspace_bytes, stream);
+}
+
+// ------------------------------------------------------------------ exact top-k for large k / many queries
+// Per chunk of queries: the wgmma GEMM writes the fp32 score block [q_chunk, ld] into the workspace
+// (gemm_scores_f32), then knn_select_kernel (knn_select.cuh) radix-selects each query's k best rows from its row.
+namespace crag {
+namespace {
+inline int64_t knn_ld(int64_t n_rows) { return ((n_rows > 0 ? n_rows : 1) + 3) & ~int64_t(3); }
+}  // namespace
+}  // namespace crag
+
+extern "C" size_t crag_knn_workspace_bytes(int64_t n_rows, int q_chunk) {
+  if (n_rows < 0 || q_chunk < 1) return 0;
+  return (size_t(q_chunk) * size_t(knn_ld(n_rows)) * 4 + 255) & ~size_t(255);
+}
+
+extern "C" int crag_knn_topk(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride, int64_t row_offset,
+                             const void* queries, int nq, int k, int64_t* out_ids, float* out_scores, float* out_minmax,
+                             void* workspace, size_t workspace_bytes, crag_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const SearchPlan no_scan_workspace{0, 0, 0, 0};
+  int rc = check_search_args(corpus, n_rows, dim, corpus_row_stride, queries, nq, k, workspace, workspace_bytes,
+                             no_scan_workspace, kKnnMaxK);
+  if (rc != CRAG_OK) return rc;
+  if (!out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "knn: null output pointer");
+  const int64_t ld = knn_ld(n_rows);
+  const size_t per_query = size_t(ld) * 4;
+  const size_t fit = workspace_bytes / per_query;
+  if (fit < 1) return fail(CRAG_ERR_WORKSPACE, "knn: workspace %zu < %zu bytes (one query's score row)", workspace_bytes, per_query);
+  const int q_chunk = fit < size_t(nq) ? int(fit) : nq;
+  float* block = static_cast<float*>(workspace);
+  for (int q0 = 0; q0 < nq; q0 += q_chunk) {
+    const int nqc = (nq - q0) < q_chunk ? (nq - q0) : q_chunk;
+    rc = gemm_scores_f32(static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, dim, corpus, corpus_row_stride,
+                         block, ld, nqc, int(n_rows), dim, stream);
+    if (rc != CRAG_OK) return rc;
+    knn_select_kernel<<<nqc, kKnnThreads, 0, stream>>>(block, ld, int(n_rows), k, row_offset, out_ids + size_t(q0) * k,
+                                                       out_scores + size_t(q0) * k,
+                                                       out_minmax ? out_minmax + size_t(q0) * 2 : nullptr);
+    CRAG_CUDA_OK(cudaGetLastError());
+  }
+  return CRAG_OK;
 }
 
 namespace crag {

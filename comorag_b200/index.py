@@ -17,11 +17,45 @@ import torch
 from . import _native
 
 MAX_DIM = 1024
-MAX_K = 128
+MAX_K = 128            # the shard scan (crag_search_topk) and everything built on it
+KNN_MAX_K = 2048       # crag_knn_topk: score-block GEMM + per-query radix select
+# Score-block budget of crag_knn_topk: a chunk holds this many bytes of fp32 scores (4 * round_up(n_rows, 4) per query)
+KNN_WORKSPACE_BYTES = 1 << 30
+# Routing between crag_knn_topk and the shard scan, from tools/knn_bench.py on an NVIDIA H100 80GB HBM3 at a 700 W
+# power limit (new path vs scan path, ms per call):
+#   self-join, N = nq = 10k / 50k / 200k, dim 384 and 1024: the new path wins at every k -- k = 10: 0.78 vs 14.0,
+#     23.0 vs 175, 389 vs 1329 (dim 1024, 200k); k = 2047: 1.97 vs 763, 26.2 vs 7326, 402 vs 54160 (dim 1024).
+#     The smallest winning batch is nq = 10 000; the smallest winning chunk holds 1 280 queries (N = 200k).
+#   N = 10M, dim 1024, nq = 1 / 32 / 256: k = 10 loses (16.6 vs 6.9, 33.5 vs 6.8, 165 vs 53), k = 2047 wins (16.6 vs
+#     114, 33.4 vs 119, 165 vs 937).  There one call of the new path costs what 2.4 / 4.9 / 3.1 scan passes cost, and
+#     the scan needs ceil(k/128) passes, so k > 640 (>= 6 passes) is on the winning side for every measured nq.
+KNN_MIN_QUERIES = 10_000    # many queries: the GEMM path for any k <= 2048 ...
+KNN_MIN_CHUNK = 1_280       # ... when a chunk of the workspace budget holds at least this many of them
+KNN_MIN_K_FEW = 641         # few queries: the GEMM path from this k on
 
 
 def _pad_dim(dim: int) -> int:
     return (dim + 63) // 64 * 64
+
+
+def knn_chunk(nq: int, n_rows: int, budget: int = KNN_WORKSPACE_BYTES) -> int:
+    """Queries per crag_knn_topk chunk whose score rows fit `budget` bytes: at least 1, at most nq, and a multiple of
+    the GEMM's 128-row tile wherever nq and the budget allow."""
+    per_query = 4 * ((max(n_rows, 1) + 3) // 4 * 4)
+    c = min(nq, max(1, budget // per_query))
+    if 128 <= c < nq:
+        c = c // 128 * 128
+    return c
+
+
+def use_knn(nq: int, n_rows: int, k: int) -> bool:
+    """Route a search to crag_knn_topk (True) or to the shard scan (False): for k <= 2048, the GEMM path for large
+    query batches whose chunks stay large, or for k >= KNN_MIN_K_FEW; the scan otherwise and always beyond k = 2048."""
+    if k > KNN_MAX_K:
+        return False
+    if nq >= KNN_MIN_QUERIES and knn_chunk(nq, n_rows) >= KNN_MIN_CHUNK:
+        return True
+    return k >= KNN_MIN_K_FEW
 
 
 class _GrowableRows:
@@ -228,9 +262,11 @@ class DenseIndex:
         """
         if k < 1:
             raise ValueError("k must be >= 1")
+        if k > MAX_K and out is not None:
+            raise ValueError(f"out= is only supported for k <= {MAX_K}")
+        if use_knn(queries.shape[0], self._n, k):
+            return self._search_device_knn(queries, k, stream, out)
         if k > MAX_K:
-            if out is not None:
-                raise ValueError(f"out= is only supported for k <= {MAX_K}")
             return self._search_device_paged(queries, k, stream)
         if queries.dtype != torch.bfloat16 or queries.dim() != 2 or queries.shape[1] != self.dim_pad:
             raise ValueError(f"queries must be bf16 [nq, {self.dim_pad}]")
@@ -259,8 +295,38 @@ class DenseIndex:
                 _native.check(rc, "crag_search_topk")
         return ids, scores, minmax
 
+    def _search_device_knn(self, queries: torch.Tensor, k: int, stream: Optional[torch.cuda.Stream], out=None):
+        """crag_knn_topk: per chunk of queries one wgmma GEMM writes the fp32 score block, one CTA per query
+        radix-selects its k best.  Same outputs as the scan path."""
+        if queries.dtype != torch.bfloat16 or queries.dim() != 2 or queries.shape[1] != self.dim_pad:
+            raise ValueError(f"queries must be bf16 [nq, {self.dim_pad}]")
+        queries = queries.contiguous()
+        nq = queries.shape[0]
+        lib = _native.load()
+        dev = self.device
+        buf, n_rows = self._snapshot()
+        with torch.cuda.device(dev):
+            st = stream if stream is not None else torch.cuda.current_stream(dev)
+            with torch.cuda.stream(st):
+                if out is not None:
+                    ids, scores, minmax = out
+                else:
+                    ids = torch.empty((nq, k), dtype=torch.int64, device=dev)
+                    scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
+                    minmax = torch.empty((nq, 2), dtype=torch.float32, device=dev)
+                ws_bytes = lib.crag_knn_workspace_bytes(n_rows, knn_chunk(nq, n_rows))
+                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+                rc = lib.crag_knn_topk(
+                    buf.data_ptr() if n_rows else 0, n_rows, self.dim_pad,
+                    buf.stride(0) if buf.shape[0] else self.dim_pad,
+                    self.row_offset, queries.data_ptr(), nq, k, ids.data_ptr(), scores.data_ptr(),
+                    minmax.data_ptr(), ws.data_ptr(), ws_bytes, st.cuda_stream)
+                _native.check(rc, "crag_knn_topk")
+        return ids, scores, minmax
+
     def _search_device_paged(self, queries: torch.Tensor, k: int, stream: Optional[torch.cuda.Stream]):
-        """k > 128: ceil(k/128) passes chained with crag_search_topk_after (exact rank continuation)."""
+        """k > 128 where crag_knn_topk does not pay off (few queries, or k > 2048): ceil(k/128) passes chained with
+        crag_search_topk_after (exact rank continuation)."""
         if queries.dtype != torch.bfloat16 or queries.dim() != 2 or queries.shape[1] != self.dim_pad:
             raise ValueError(f"queries must be bf16 [nq, {self.dim_pad}]")
         queries = queries.contiguous()

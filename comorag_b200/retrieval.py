@@ -112,8 +112,11 @@ def retrieve_knn(query_ids: List[str], key_ids: List[str], query_vecs, key_vecs,
 
     The reference L2-normalises both sides and does blocked torch.mm + torch.topk with a two-stage merge, i.e. the
     exact top-min(k, #keys) per query, scores descending.  Here the normalised keys become a bf16 device shard and
-    the queries run through the fused kernel, 128 ranks per pass chained with crag_search_topk_after.  The two batch
-    size arguments are accepted for signature compatibility; blocking is the kernel's own.
+    every group of queries goes through DenseIndex.search: for k <= 2048 and a full group (the self-join of
+    add_synonymy_edges, ComoRAG.py:670-684) that is crag_knn_topk -- one wgmma GEMM per chunk of queries writing the
+    fp32 score block, then a per-query radix select --, otherwise the fused scan, 128 ranks per pass chained with
+    crag_search_topk_after.  The two batch size arguments are accepted for signature compatibility; blocking is the
+    library's own.
     """
     import torch
     if len(key_vecs) == 0:

@@ -107,6 +107,19 @@ CRAG_API int crag_search_topk_after(const void* corpus, int64_t n_rows, int dim,
                                     int64_t* out_ids, float* out_scores, float* out_minmax, uint64_t* last_keys,
                                     void* workspace, size_t workspace_bytes, crag_stream_t stream);
 
+/* Exact top-k for large k and/or many queries: per chunk of queries one wgmma GEMM writes the fp32 score block
+ * [q_chunk, round_up(n_rows, 4)] into the workspace, then one CTA per query radix-selects its k best.
+ * Same argument rules and the same output contract as crag_search_topk (score desc, ties by ascending row, -1/-inf
+ * past n_rows, minmax over all rows), except 1 <= k <= 2048.  q_chunk = workspace_bytes / per-query bytes (>= 1,
+ * else CRAG_ERR_WORKSPACE); the call loops over chunks.  The self-join of the reference's add_synonymy_edges
+ * (ComoRAG.py:670-684 -> retrieve_knn, embed_utils.py:8-97, k = 2047) is one GEMM per chunk instead of
+ * ceil(nq/32) * ceil(k/128) passes over the shard.  Workspace 256-B aligned; crag_knn_workspace_bytes(n_rows, q)
+ * is the size that holds q queries' score rows. */
+CRAG_API size_t crag_knn_workspace_bytes(int64_t n_rows, int q_chunk);
+CRAG_API int crag_knn_topk(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride, int64_t row_offset,
+                           const void* queries, int nq, int k, int64_t* out_ids, float* out_scores, float* out_minmax,
+                           void* workspace, size_t workspace_bytes, crag_stream_t stream);
+
 /* The two halves of crag_search_topk for ONE pass (nq <= 32), exported so a caller can time or overlap them:
  * crag_search_scan streams the shard once and leaves per-CTA partial lists in the workspace;
  * crag_search_finalize merges them into (ids, scores, minmax).  Same argument rules as crag_search_topk. */
