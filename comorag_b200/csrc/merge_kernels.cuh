@@ -14,11 +14,51 @@
 namespace crag {
 
 // ---------------------------------------------------------------------------
-// Merge kernels: one warp per query streams candidate keys through the same
+// Two-level merge of `parts` sorted lists of k keys, fetch(p, j) = key j of list p (0 = absent), by one CTA of 4 warps:
+// warp w streams lists w, w + 4, ... through its selector into s_keys[w], then warp 0 merges the four into s_keys[4].
+// Keys below `bound` are skipped up front.  Returns true in warp 0, the warp that holds the result.
+template <int KLIST, int CAP, class Fetch>
+__device__ __forceinline__ bool merge_lists(uint64_t (&s_keys)[5][KLIST + CAP], uint64_t (&s_thr)[5], int parts, int k,
+                                            uint64_t bound, Fetch fetch) {
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int my_parts = parts > w ? (parts - w + 3) / 4 : 0;
+  select_stream<KLIST, CAP>(s_keys[w], &s_thr[w], lane, k, my_parts * k, bound, [&](int idx) -> uint64_t {
+    const int pl = idx / k, j = idx - pl * k;
+    return fetch(w + 4 * pl, j);
+  });
+  __syncthreads();
+  if (w != 0) return false;
+  select_stream<KLIST, CAP>(s_keys[4], &s_thr[4], lane, k, 4 * k, 0ull, [&](int idx) -> uint64_t { return s_keys[idx / k][idx % k]; });
+  return true;
+}
+
+// Query q's top-k over the per-CTA lists of a scan, part_keys[(p * q_stride + q) * k + j] for p < parts, into s_keys[4].
+// Returns true in warp 0, the warp that holds the result.
+template <int KLIST, int CAP>
+__device__ __forceinline__ bool merge_cta_lists(uint64_t (&s_keys)[5][KLIST + CAP], uint64_t (&s_thr)[5], const uint64_t* __restrict__ part_keys,
+                                                int q_stride, int q, int parts, int k) {
+  // Admission bound before any sorting: every part's list is sorted, so its k-th entry is a lower bound of the
+  // global k-th best (that part alone already holds k candidates at least that good); the max over parts rejects
+  // almost all of the parts*k candidates up front.
+  const int lane = threadIdx.x & 31;
+  uint64_t bound = 0;
+  for (int p = lane; p < parts; p += 32) {
+    const uint64_t kth = part_keys[(size_t(p) * q_stride + q) * k + (k - 1)];
+    bound = kth > bound ? kth : bound;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const uint64_t other = shfl_xor_u64(bound, o);
+    bound = other > bound ? other : bound;
+  }
+  return merge_lists<KLIST, CAP>(s_keys, s_thr, parts, k, bound, [&](int p, int j) { return part_keys[(size_t(p) * q_stride + q) * k + j]; });
+}
+
+// ---------------------------------------------------------------------------
+// Merge kernels: one CTA per query streams candidate keys through the same
 // selector.  PAIRS=false: raw keys (local row ids) from search_topk_kernel's
 // CTAs, ids are widened and offset on output.  PAIRS=true: (score, int64 id)
 // pairs from several shards; ties resolve by candidate position.
-// One CTA (4 warps) per query: warp w merges parts w, w+4, ... into its own list, warp 0 merges the four lists.
 template <int KLIST, int CAP, bool PAIRS>
 __global__ void __launch_bounds__(128) merge_topk_kernel(const uint64_t* __restrict__ part_keys,
                                                          const float* __restrict__ in_scores,
@@ -33,40 +73,22 @@ __global__ void __launch_bounds__(128) merge_topk_kernel(const uint64_t* __restr
   constexpr int KPQ = KLIST + CAP;
   __shared__ uint64_t s_keys[5][KPQ];
   __shared__ uint64_t s_thr[5];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int q = blockIdx.x;
 
-  // Admission bound before any sorting: every part's list is sorted, so its k-th entry is a lower bound of the
-  // global k-th best (that part alone already holds k candidates at least that good); the max over parts rejects
-  // almost all of the parts*k candidates up front.
-  uint64_t bound = 0;
-  if (!PAIRS) {
-    for (int p = lane; p < parts; p += 32) {
-      const uint64_t kth = part_keys[(size_t(p) * q_stride + q) * k + (k - 1)];
-      bound = kth > bound ? kth : bound;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const uint64_t other = shfl_xor_u64(bound, o);
-      bound = other > bound ? other : bound;
-    }
-  }
-  const int my_parts = parts > w ? (parts - w + 3) / 4 : 0;
-  select_stream<KLIST, CAP>(s_keys[w], &s_thr[w], lane, k, my_parts * k, bound, [&](int idx) -> uint64_t {
-    const int pl = idx / k, j = idx - pl * k, p = w + 4 * pl;
-    if (PAIRS) {
+  bool merged;
+  if constexpr (PAIRS) {
+    merged = merge_lists<KLIST, CAP>(s_keys, s_thr, parts, k, 0ull, [&](int p, int j) -> uint64_t {
       const size_t at = size_t(q) * k + j;
       const int64_t id = *reinterpret_cast<const int64_t*>(reinterpret_cast<const char*>(in_ids + at) + p * ids_stride);
       const float sc = *reinterpret_cast<const float*>(reinterpret_cast<const char*>(in_scores + at) + p * scores_stride);
       return id >= 0 ? make_key(sc, uint32_t(p * k + j)) : 0ull;
-    }
-    return part_keys[(size_t(p) * q_stride + q) * k + j];
-  });
-  __syncthreads();
-  if (w != 0) return;
+    });
+  } else {
+    merged = merge_cta_lists<KLIST, CAP>(s_keys, s_thr, part_keys, q_stride, q, parts, k);
+  }
+  if (!merged) return;
   uint64_t* keys = s_keys[4];
-  select_stream<KLIST, CAP>(keys, &s_thr[4], lane, k, 4 * k, 0ull,
-                            [&](int idx) -> uint64_t { return s_keys[idx / k][idx % k]; });
   for (int j = lane; j < k; j += 32) {
     const uint64_t key = keys[j];
     float s = -INFINITY;
@@ -95,11 +117,7 @@ __global__ void __launch_bounds__(128) merge_topk_kernel(const uint64_t* __restr
         b = fmaxf(b, mm[1]);
       }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      a = fminf(a, __shfl_xor_sync(0xffffffffu, a, o));
-      b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
-    }
+    warp_minmax(a, b);
     if (lane == 0) {
       out_minmax[size_t(q) * 2 + 0] = a;
       out_minmax[size_t(q) * 2 + 1] = b;
@@ -110,7 +128,7 @@ __global__ void __launch_bounds__(128) merge_topk_kernel(const uint64_t* __restr
 // ---------------------------------------------------------------------------
 // Fused per-shard finalize + cross-rank exchange + global merge for the row-sharded index (SURVEY.md section 8e), over
 // NVLink peer memory instead of an NCCL all-gather launch.  One CTA per query:
-//   1. merge this rank's per-CTA partial lists into the shard's top-k (as merge_topk_kernel does);
+//   1. merge this rank's per-CTA partial lists into the shard's top-k (merge_cta_lists, as merge_topk_kernel);
 //   2. PUSH the k (id, score) pairs + (min, max) into slot [parity][this rank][q] of EVERY rank's exchange buffer
 //      (peer-mapped symmetric memory: plain stores that travel over NVLink), fence, then release-store the epoch
 //      into flag [parity][this rank][q] of every rank;
@@ -167,35 +185,13 @@ __global__ void __launch_bounds__(128) finalize_exchange_kernel(const uint64_t* 
   if (threadIdx.x == 0) s_bad = 0;
 
   // ---- 1. this shard's top-k for query q (parts may be 0: empty shard)
-  uint64_t bound = 0;
-  for (int p = lane; p < parts; p += 32) {
-    const uint64_t kth = part_keys[(size_t(p) * kNQ + q) * k + (k - 1)];
-    bound = kth > bound ? kth : bound;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const uint64_t other = shfl_xor_u64(bound, o);
-    bound = other > bound ? other : bound;
-  }
-  const int my_parts = parts > w ? (parts - w + 3) / 4 : 0;
-  select_stream<KLIST, CAP>(s_keys[w], &s_thr[w], lane, k, my_parts * k, bound, [&](int idx) -> uint64_t {
-    const int pl = idx / k, j = idx - pl * k, p = w + 4 * pl;
-    return part_keys[(size_t(p) * kNQ + q) * k + j];
-  });
-  __syncthreads();
-  if (w == 0) {
-    select_stream<KLIST, CAP>(s_keys[4], &s_thr[4], lane, k, 4 * k, 0ull,
-                              [&](int idx) -> uint64_t { return s_keys[idx / k][idx % k]; });
+  if (merge_cta_lists<KLIST, CAP>(s_keys, s_thr, part_keys, kNQ, q, parts, k)) {
     float a = INFINITY, b = -INFINITY;
     for (int p = lane; p < parts; p += 32) {
       a = fminf(a, part_minmax[(size_t(p) * kNQ + q) * 2 + 0]);
       b = fmaxf(b, part_minmax[(size_t(p) * kNQ + q) * 2 + 1]);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      a = fminf(a, __shfl_xor_sync(0xffffffffu, a, o));
-      b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
-    }
+    warp_minmax(a, b);
     if (lane == 0) { s_mm[0] = a; s_mm[1] = b; }
   }
   __syncthreads();
@@ -273,11 +269,7 @@ __global__ void __launch_bounds__(128) finalize_exchange_kernel(const uint64_t* 
       a = __ldcv(mm);
       b = __ldcv(mm + 1);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      a = fminf(a, __shfl_xor_sync(0xffffffffu, a, o));
-      b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
-    }
+    warp_minmax(a, b);
     if (lane == 0) {
       out_minmax[size_t(q) * 2 + 0] = a;
       out_minmax[size_t(q) * 2 + 1] = b;

@@ -179,22 +179,4 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs_bmn(float (&d)[32], const uin
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
 }
 
-// Named barrier among a subset of the CTA's warps (id 1..15; 0 is __syncthreads).
-__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
-  asm volatile("barrier.cta.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-// Barrier + OR-reduction of a predicate over the participating threads.
-__device__ __forceinline__ bool named_bar_or(uint32_t id, uint32_t nthreads, bool pred) {
-  uint32_t out;
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %1, 0;\n\t"
-      "barrier.cta.red.or.pred q, %2, %3, p;\n\t"
-      "selp.u32 %0, 1, 0, q;\n\t}"
-      : "=r"(out)
-      : "r"(static_cast<uint32_t>(pred)), "r"(id), "r"(nthreads)
-      : "memory");
-  return out != 0;
-}
-
 }  // namespace crag

@@ -32,6 +32,8 @@
 // (finalize_exchange_kernel), the C-ABI entry points, and crag_knn_topk -- exact
 // top-k up to k = 2048 for large query batches as a score-block GEMM (gemm.cu)
 // plus a per-query radix select (knn_select.cuh).
+#include <type_traits>
+
 #include "common.cuh"
 #include "ptx.cuh"
 #include "topk.cuh"
@@ -39,10 +41,22 @@
 #include "merge_kernels.cuh"
 #include "ivf_kernels.cuh"
 #include "search_types.cuh"
+#include "select_warps.cuh"
 #include "gemm.cuh"
 #include "knn_select.cuh"
 
 namespace crag {
+
+// Dynamic shared memory of the scan, from a 1024-byte aligned base: the pipeline stages, the score tiles, the
+// selector (select_warps.cuh), then the mbarriers.
+template <int KLIST, int CAP, int STAGES>
+struct SearchLayout {
+  static constexpr size_t kTilesOff = size_t(STAGES) * kStageTotalBytes;
+  static constexpr size_t kSelectOff = kTilesOff + size_t(kAccStages) * kScoreTileBytes;
+  static constexpr size_t kBarsOff = kSelectOff + SelectSmem<KLIST, CAP>::bytes();
+  // + the alignment pad of the base and 16 bytes of slack past the mbarriers
+  __host__ __device__ static constexpr size_t smem_bytes() { return 1024 + kBarsOff + (2 * STAGES + 2 * kAccStages) * 8 + 16; }
+};
 
 // the 32 scores of row `row` of a score tile (layout: score_slot) -> r[q]
 __device__ __forceinline__ void ld_score_row(const float* tile, int row, uint32_t (&r)[kNQ]) {
@@ -50,47 +64,47 @@ __device__ __forceinline__ void ld_score_row(const float* tile, int row, uint32_
   for (int q = 0; q < kNQ; ++q) r[q] = __float_as_uint(tile[score_slot(row, q)]);
 }
 
+// The select warps' score-tile source: wait until the wgmma warpgroup has filled score tile `acc`, read this lane's
+// row of it, and hand the buffer back once the whole warp has read.
+struct SmemScoreTiles {
+  const float* tiles;            // [kAccStages][128 * 32]
+  uint64_t *full, *empty;        // [kAccStages] each
+  int acc = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void next(int /*tile*/, int quad, int lane, uint32_t (&r)[kNQ]) {
+    mbar_wait(&full[acc], phase);
+    ld_score_row(tiles + acc * (kTileRows * kNQ), quad * 32 + lane, r);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[acc]);
+    if (++acc == kAccStages) { acc = 0; phase ^= 1; }
+  }
+};
+
 template <int KLIST, int CAP, int STAGES, bool IVF = false, bool SCORES = false>
 __global__ void __launch_bounds__(kSearchThreads, 1)
 search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_constant__ CUtensorMap tm_q,
                    int n_rows, int num_kb, int nq, int k, const uint64_t* __restrict__ after_keys,
                    uint64_t* __restrict__ pool, uint32_t perm_mul, int perm_shift, uint64_t* __restrict__ part_keys,
-                   float* __restrict__ part_minmax, const typename IvfParam<IVF, SCORES>::type ivf) {
+                   float* __restrict__ part_minmax, const typename IvfParam<IVF, SCORES>::type args) {
   using L = SearchLayout<KLIST, CAP, STAGES>;
   static_assert(L::smem_bytes() <= 227 * 1024, "stages, score tiles and candidate lists exceed 227 KB of shared memory");
-  constexpr int kAccStages = L::kAccStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
   uint8_t* stage_base = smem;
-  float* score_tiles = reinterpret_cast<float*>(stage_base + STAGES * kStageTotalBytes);   // [kAccStages][128 * 32]
-  uint64_t* keys = reinterpret_cast<uint64_t*>(stage_base + STAGES * kStageTotalBytes + kAccStages * kScoreTileBytes);
-  uint64_t* bar_full = keys + kNQ * L::kKeysPerQuery;
+  float* score_tiles = reinterpret_cast<float*>(smem + L::kTilesOff);
+  const auto sel = SelectSmem<KLIST, CAP>::carve(smem + L::kSelectOff);
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + L::kBarsOff);
   uint64_t* bar_empty = bar_full + STAGES;
   uint64_t* bar_tfull = bar_empty + STAGES;            // [kAccStages]
   uint64_t* bar_tempty = bar_tfull + kAccStages;       // [kAccStages]
-  uint64_t* thr_key = bar_tempty + kAccStages;         // [kNQ]
-  float* thr_f = reinterpret_cast<float*>(thr_key + kNQ);  // [kNQ]
-  int* cnt = reinterpret_cast<int*>(thr_f + kNQ);          // [kNQ]
-  float* red = reinterpret_cast<float*>(cnt + kNQ);        // [4][kNQ][2]
-  uint64_t* bnd_key = reinterpret_cast<uint64_t*>(red + 4 * kNQ * 2);  // [kNQ] admit only keys < bnd_key
-  float* bnd_f = reinterpret_cast<float*>(bnd_key + kNQ);              // [kNQ] score part of the bound
-  uint64_t* floor_key = reinterpret_cast<uint64_t*>(bnd_f + kNQ);      // [kNQ] pooled admission floor (see kPoolM)
-  uint64_t* part_floor = floor_key + kNQ;                              // [4][kNQ] scratch of a floor refresh
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   int num_tiles;
-  if constexpr (IVF) num_tiles = __ldg(ivf.n_work);
+  if constexpr (IVF) num_tiles = __ldg(args.n_work);
   else num_tiles = (n_rows + kTileRows - 1) / kTileRows;
-
-  // Flat scans walk GROUPS of 2^perm_shift consecutive tiles in a multiplicative permutation of the row order
-  // (perm_mul coprime to the number of whole groups; a ragged tail keeps its place): at any moment the CTAs sample the
-  // whole shard, so a corpus whose scores drift along the row order (rows appended in narrative order, planted
-  // neighbours in the tail) looks like a random one to the selector.  Neighbouring CTAs still stream neighbouring
-  // tiles of one group (2 MB at shift 3 = one page of address translation), which is what HBM and the TLBs like.
-#define CRAG_SELECT_SECTION 1
-#include "select_warps.inc.cuh"
+  const TileOrder order(num_tiles, perm_mul, perm_shift);
 
   // ------------------------------------------------------------ one-time setup
   if (threadIdx.x == 0) {
@@ -104,8 +118,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
     }
     fence_mbar_init();
   }
-#define CRAG_SELECT_SECTION 2
-#include "select_warps.inc.cuh"
+  sel.init(nq, after_keys);
   __syncthreads();
 
   if (warp == kProducerWarp) {
@@ -117,12 +130,12 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
       int stage = 0;
       uint32_t phase = 0;
       for (int j = blockIdx.x; j < num_tiles; j += gridDim.x) {
-        const int tile = tile_of(j);
+        const int tile = IVF ? j : order(j);
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&bar_empty[stage], phase ^ 1);
           mbar_arrive_expect_tx(&bar_full[stage], kStageTotalBytes);
           int tile_row0;
-          if constexpr (IVF) tile_row0 = __ldg(&ivf.work[tile].x);
+          if constexpr (IVF) tile_row0 = __ldg(&args.work[tile].x);
           else tile_row0 = tile * kTileRows;
           uint8_t* st = stage_base + stage * kStageTotalBytes;
           tma_load_2d_hint(&tm_corpus, &bar_full[stage], st, kb * kBlockK, tile_row0, pol);
@@ -182,8 +195,8 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
     }
   } else {
     // ================================================================== select
-#define CRAG_SELECT_SECTION 3
-#include "select_warps.inc.cuh"
+    SmemScoreTiles tiles{score_tiles, bar_tfull, bar_tempty};
+    select_warps<KLIST, CAP, IVF, SCORES>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, args, warp, lane);
   }
 }
 
@@ -207,47 +220,45 @@ SearchPlan plan_search(int k) {
   return p;
 }
 
-// cudaFuncSetAttribute once per kernel and device instead of on every launch.  `Tag` makes the cache unique per
-// kernel instantiation (the kernels share one function-pointer TYPE, so the pointer type alone would alias them).
-template <class Tag, class Kern>
-int ensure_smem_attr(Kern kern, size_t smem) {
-  static size_t done[64] = {0};
+// One launch of the scan.  The dynamic shared-memory limit is raised once per instantiation and device.
+template <int KLIST, int CAP, int STAGES, bool IVF, bool SCORES>
+int launch_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k, int grid,
+                const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift, uint64_t* part_keys,
+                float* part_minmax, const typename IvfParam<IVF, SCORES>::type& args, cudaStream_t stream) {
+  constexpr size_t smem = SearchLayout<KLIST, CAP, STAGES>::smem_bytes();
+  auto kern = search_topk_kernel<KLIST, CAP, STAGES, IVF, SCORES>;
+  static bool attr_set[64] = {};
   int dev = 0;
   CRAG_CUDA_OK(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64 || done[dev] < smem) {
+  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
     CRAG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-    if (dev >= 0 && dev < 64) done[dev] = smem;
+    if (dev >= 0 && dev < 64) attr_set[dev] = true;
   }
-  return CRAG_OK;
-}
-template <int KLIST, int CAP, int STAGES, bool IVF, bool SCORES> struct KernelTag {};
-
-template <int KLIST, int CAP, int STAGES>
-int launch_search(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k,
-                  int grid, const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift,
-                  uint64_t* part_keys, float* part_minmax, cudaStream_t stream) {
-  using L = SearchLayout<KLIST, CAP, STAGES>;
-  const size_t smem = L::smem_bytes();
-  auto kern = search_topk_kernel<KLIST, CAP, STAGES>;
-  int rc = ensure_smem_attr<KernelTag<KLIST, CAP, STAGES, false, false>>(kern, smem);
-  if (rc != CRAG_OK) return rc;
-  kern<<<grid, kSearchThreads, smem, stream>>>(tm_corpus, tm_q, n_rows, num_kb, nq, k, after_keys, pool, perm_mul,
-                                               perm_shift, part_keys, part_minmax, NoIvfArgs{});
+  kern<<<grid, kSearchThreads, smem, stream>>>(tm_corpus, tm_q, n_rows, num_kb, nq, k, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }
 
-template <int KLIST, int CAP, int STAGES>
-int launch_ivf_scan(const CUtensorMap& tm_res, const CUtensorMap& tm_q, int num_kb, int nq, int k, int grid,
-                    uint64_t* pool, uint64_t* part_keys, float* part_minmax, const IvfArgs& ivf, cudaStream_t stream) {
-  using L = SearchLayout<KLIST, CAP, STAGES>;
-  const size_t smem = L::smem_bytes();
-  auto kern = search_topk_kernel<KLIST, CAP, STAGES, true>;
-  int rc = ensure_smem_attr<KernelTag<KLIST, CAP, STAGES, true, false>>(kern, smem);
-  if (rc != CRAG_OK) return rc;
-  kern<<<grid, kSearchThreads, smem, stream>>>(tm_res, tm_q, 0, num_kb, nq, k, nullptr, pool, 0u, 0, part_keys, part_minmax, ivf);
-  CRAG_CUDA_OK(cudaGetLastError());
-  return CRAG_OK;
+// A top-k scan with the selector of k: 64-key lists and 6 stages up to k = 64, 128-key lists and 4 stages above.
+template <bool IVF, class Args>
+int launch_topk_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k,
+                     int grid, const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift,
+                     uint64_t* part_keys, float* part_minmax, const Args& args, cudaStream_t stream) {
+  if (k <= 64) return launch_scan<64, 64, 6, IVF, false>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+  return launch_scan<128, 128, 4, IVF, false>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+}
+
+// The merge kernels' list size for k (32, 64 or 128), passed to `launch` as a std::integral_constant.
+template <class Launch>
+void with_merge_tier(int k, Launch launch) {
+  if (k <= 32) launch(std::integral_constant<int, 32>{});
+  else if (k <= 64) launch(std::integral_constant<int, 64>{});
+  else launch(std::integral_constant<int, 128>{});
+}
+
+// tensor map of queries q0 .. q0 + nqc - 1 (nqc <= 32) of a dense [nq, dim] bf16 array
+int make_query_tmap(CUtensorMap* tm, const void* queries, int q0, int nqc, int dim) {
+  return make_tmap_bf16_2d(tm, static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, uint64_t(nqc), uint64_t(dim), uint64_t(dim) * 2, kNQ);
 }
 
 }  // namespace
@@ -284,10 +295,13 @@ inline int scan_grid(int64_t n_rows, const SearchPlan& plan) {
   return num_tiles < plan.grid ? num_tiles : plan.grid;
 }
 
-// one corpus pass for <= 32 queries: per-CTA partial lists into the workspace
-int scan_pass(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride, const void* queries, int nq,
-              int k, const uint64_t* after_keys, void* workspace, size_t workspace_bytes, const SearchPlan& plan,
-              cudaStream_t stream) {
+// the flat scans permute groups of 2^kPermShift consecutive tiles (TileOrder)
+constexpr int kPermShift = 3;
+
+// one corpus pass for queries q0 .. q0 + nq - 1 (nq <= 32): per-CTA partial lists into the workspace
+int scan_pass(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride, const void* queries, int q0,
+              int nq, int k, const uint64_t* after_keys, void* workspace, size_t workspace_bytes,
+              const SearchPlan& plan, cudaStream_t stream) {
   const int grid = scan_grid(n_rows, plan);
   if (grid == 0) return CRAG_OK;
   uint64_t* part_keys = static_cast<uint64_t*>(workspace);
@@ -302,17 +316,10 @@ int scan_pass(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_st
   CUtensorMap tm_corpus, tm_q;
   int rc = make_tmap_bf16_2d(&tm_corpus, corpus, uint64_t(n_rows), uint64_t(dim), uint64_t(corpus_row_stride) * 2, kTileRows);
   if (rc != CRAG_OK) return rc;
-  rc = make_tmap_bf16_2d(&tm_q, queries, uint64_t(nq), uint64_t(dim), uint64_t(dim) * 2, kNQ);
+  rc = make_query_tmap(&tm_q, queries, q0, nq, dim);
   if (rc != CRAG_OK) return rc;
-  const int num_kb = dim / kBlockK;
-  // A/B switches for measurements (read once): CRAG_SEARCH_PERM_SHIFT = -1 (natural order) | 0..6, CRAG_SEARCH_POOL = 0
-  static const int env_shift = [] { const char* e = getenv("CRAG_SEARCH_PERM_SHIFT"); return e ? atoi(e) : 3; }();
-  static const bool env_pool = [] { const char* e = getenv("CRAG_SEARCH_POOL"); return e ? atoi(e) != 0 : true; }();
-  if (!env_pool) pool = nullptr;
-  const int shift = env_shift < 0 ? 0 : (env_shift > 6 ? 6 : env_shift);
-  const uint32_t perm = env_shift < 0 ? 0u : perm_multiplier(num_tiles >> shift);
-  if (k <= 64) return launch_search<64, 64, 6>(tm_corpus, tm_q, int(n_rows), num_kb, nq, k, grid, after_keys, pool, perm, shift, part_keys, part_minmax, stream);
-  return launch_search<128, 128, 4>(tm_corpus, tm_q, int(n_rows), num_kb, nq, k, grid, after_keys, pool, perm, shift, part_keys, part_minmax, stream);
+  return launch_topk_scan<false>(tm_corpus, tm_q, int(n_rows), dim / kBlockK, nq, k, grid, after_keys, pool,
+                                 perm_multiplier(num_tiles >> kPermShift), kPermShift, part_keys, part_minmax, NoIvfArgs{}, stream);
 }
 
 // merge the per-CTA partials of one pass into the final (ids, scores, minmax) of its <= 32 queries
@@ -320,13 +327,11 @@ int finalize_parts(const void* workspace, int grid, int nq, int k, int64_t row_o
                    float* out_scores, float* out_minmax, uint64_t* last_keys, const SearchPlan& plan, cudaStream_t stream) {
   const uint64_t* part_keys = static_cast<const uint64_t*>(workspace);
   const float* part_minmax = reinterpret_cast<const float*>(static_cast<const uint8_t*>(workspace) + plan.keys_bytes);
-  const int mgrid = nq;  // one CTA per query
-  if (k <= 32)
-    merge_topk_kernel<32, 32, false><<<mgrid, 128, 0, stream>>>(part_keys, nullptr, nullptr, part_minmax, grid, kNQ, nq, k, row_offset, 0, 0, 0, out_ids, out_scores, out_minmax, last_keys);
-  else if (k <= 64)
-    merge_topk_kernel<64, 64, false><<<mgrid, 128, 0, stream>>>(part_keys, nullptr, nullptr, part_minmax, grid, kNQ, nq, k, row_offset, 0, 0, 0, out_ids, out_scores, out_minmax, last_keys);
-  else
-    merge_topk_kernel<128, 128, false><<<mgrid, 128, 0, stream>>>(part_keys, nullptr, nullptr, part_minmax, grid, kNQ, nq, k, row_offset, 0, 0, 0, out_ids, out_scores, out_minmax, last_keys);
+  with_merge_tier(k, [&](auto tier) {   // one CTA per query
+    constexpr int T = decltype(tier)::value;
+    merge_topk_kernel<T, T, false><<<nq, 128, 0, stream>>>(part_keys, nullptr, nullptr, part_minmax, grid, kNQ, nq, k, row_offset, 0, 0, 0,
+                                                           out_ids, out_scores, out_minmax, last_keys);
+  });
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }
@@ -392,7 +397,7 @@ extern "C" int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int
   for (int q0 = 0; q0 < nq; q0 += kNQ) {
     const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
     CUtensorMap tm_q;
-    rc = make_tmap_bf16_2d(&tm_q, static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, uint64_t(nqc), uint64_t(dim), uint64_t(dim) * 2, kNQ);
+    rc = make_query_tmap(&tm_q, queries, q0, nqc, dim);
     if (rc != CRAG_OK) return rc;
     ivf_plan_kernel<<<1, 1024, 0, stream>>>(probed_ids + size_t(q0) * nprobe, probed_scores + size_t(q0) * nprobe, nqc, nprobe,
                                             nlist, list_tile_start, list_rows, const_cast<uint32_t*>(ivf.list_mask),
@@ -404,8 +409,7 @@ extern "C" int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int
       pool = reinterpret_cast<uint64_t*>(ws + ip.pool_off);
       CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, sp.pool_bytes, stream));
     }
-    rc = (k <= 64) ? launch_ivf_scan<64, 64, 6>(tm_res, tm_q, num_kb, nqc, k, sp.grid, pool, part_keys, part_minmax, ivf, stream)
-                   : launch_ivf_scan<128, 128, 4>(tm_res, tm_q, num_kb, nqc, k, sp.grid, pool, part_keys, part_minmax, ivf, stream);
+    rc = launch_topk_scan<true>(tm_res, tm_q, 0, num_kb, nqc, k, sp.grid, nullptr, pool, 0u, 0, part_keys, part_minmax, ivf, stream);
     if (rc != CRAG_OK) return rc;
     rc = finalize_parts(workspace, sp.grid, nqc, k, 0, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
                         out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, nullptr, sp, stream);
@@ -423,7 +427,7 @@ extern "C" int crag_search_scan(const void* corpus, int64_t n_rows, int dim, int
   int rc = check_search_args(corpus, n_rows, dim, corpus_row_stride, queries, nq, k, workspace, workspace_bytes, plan);
   if (rc != CRAG_OK) return rc;
   if (nq > kNQ) return fail(CRAG_ERR_INVALID, "crag_search_scan handles one pass of at most %d queries (nq=%d)", kNQ, nq);
-  return scan_pass(corpus, n_rows, dim, corpus_row_stride, queries, nq, k, nullptr, workspace, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
+  return scan_pass(corpus, n_rows, dim, corpus_row_stride, queries, 0, nq, k, nullptr, workspace, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int crag_search_finalize(const void* workspace, size_t workspace_bytes, int64_t n_rows, int nq, int k,
@@ -448,9 +452,7 @@ extern "C" int crag_search_topk_after(const void* corpus, int64_t n_rows, int di
   if (!out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "search: null output pointer");
   for (int q0 = 0; q0 < nq; q0 += kNQ) {
     const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
-    const uint8_t* qptr = static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2;
-    rc = scan_pass(corpus, n_rows, dim, corpus_row_stride, qptr, nqc, k, after_keys ? after_keys + q0 : nullptr, workspace,
-                   workspace_bytes, plan, stream);
+    rc = scan_pass(corpus, n_rows, dim, corpus_row_stride, queries, q0, nqc, k, after_keys ? after_keys + q0 : nullptr, workspace, workspace_bytes, plan, stream);
     if (rc != CRAG_OK) return rc;
     rc = finalize_pass(workspace, n_rows, nqc, k, row_offset, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
                        out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, last_keys ? last_keys + q0 : nullptr, plan, stream);
@@ -516,14 +518,12 @@ int merge_pairs(const float* scores, const int64_t* ids, const float* minmax, in
                 cudaStream_t stream) {
   if (parts < 0 || nq < 1 || k < 1 || k > 128 || int64_t(parts) * k > (1 << 20)) return fail(CRAG_ERR_INVALID, "crag_merge_topk: bad sizes (parts=%d nq=%d k=%d)", parts, nq, k);
   if (!out_ids || !out_scores || (parts > 0 && (!scores || !ids))) return fail(CRAG_ERR_INVALID, "crag_merge_topk: null pointer");
-  const int mgrid = nq;  // one CTA per query
   const float* mm = out_minmax ? minmax : nullptr;
-  if (k <= 32)
-    merge_topk_kernel<32, 32, true><<<mgrid, 128, 0, stream>>>(nullptr, scores, ids, mm, parts, nq, nq, k, 0, ids_stride, scores_stride, mm_stride, out_ids, out_scores, out_minmax, nullptr);
-  else if (k <= 64)
-    merge_topk_kernel<64, 64, true><<<mgrid, 128, 0, stream>>>(nullptr, scores, ids, mm, parts, nq, nq, k, 0, ids_stride, scores_stride, mm_stride, out_ids, out_scores, out_minmax, nullptr);
-  else
-    merge_topk_kernel<128, 128, true><<<mgrid, 128, 0, stream>>>(nullptr, scores, ids, mm, parts, nq, nq, k, 0, ids_stride, scores_stride, mm_stride, out_ids, out_scores, out_minmax, nullptr);
+  with_merge_tier(k, [&](auto tier) {   // one CTA per query
+    constexpr int T = decltype(tier)::value;
+    merge_topk_kernel<T, T, true><<<nq, 128, 0, stream>>>(nullptr, scores, ids, mm, parts, nq, nq, k, 0, ids_stride, scores_stride, mm_stride,
+                                                          out_ids, out_scores, out_minmax, nullptr);
+  });
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }
@@ -560,27 +560,18 @@ __global__ void minmax_reduce_kernel(const float* __restrict__ part_minmax, int 
     a = fminf(a, part_minmax[(size_t(p) * kNQ + q) * 2 + 0]);
     b = fmaxf(b, part_minmax[(size_t(p) * kNQ + q) * 2 + 1]);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    a = fminf(a, __shfl_xor_sync(0xffffffffu, a, o));
-    b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
-  }
+  warp_minmax(a, b);
   if (lane == 0) {
     out[size_t(q) * 2 + 0] = a;
     out[size_t(q) * 2 + 1] = b;
   }
 }
-}  // namespace
-}  // namespace crag
 
-extern "C" int crag_search_scores(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,
-                                  const void* queries, int nq, float* out_scores, int64_t out_ld, float* out_minmax,
-                                  void* workspace, size_t workspace_bytes, crag_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const SearchPlan plan = plan_search(1);
-  int rc = check_search_args(corpus, n_rows, dim, corpus_row_stride, queries, nq, 1, workspace, workspace_bytes, plan);
-  if (rc != CRAG_OK) return rc;
-  if (!out_scores || out_ld < n_rows) return fail(CRAG_ERR_INVALID, "crag_search_scores: need out_scores and out_ld >= n_rows");
+// Score-all passes (the scan with SCORES), one per block of 32 queries.  Block q0 stores its scores from row q0 of
+// sa.out on, or, in assignment mode (sa.best_id set), updates every row's running argmax with ids counted from q0.
+// out_minmax (may be null) receives each query's (min, max).
+int score_passes(const void* corpus, int64_t n_rows, int dim, int64_t row_stride, const void* queries, int nq,
+                 ScoreArgs sa, float* out_minmax, void* workspace, const SearchPlan& plan, cudaStream_t stream) {
   const int grid = scan_grid(n_rows, plan);
   if (grid == 0) {
     if (out_minmax) {   // empty shard: (+inf, -inf), as crag_search_topk
@@ -591,29 +582,37 @@ extern "C" int crag_search_scores(const void* corpus, int64_t n_rows, int dim, i
   }
   float* part_minmax = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + plan.keys_bytes);
   CUtensorMap tm_corpus;
-  rc = make_tmap_bf16_2d(&tm_corpus, corpus, uint64_t(n_rows), uint64_t(dim), uint64_t(corpus_row_stride) * 2, kTileRows);
-  if (rc != CRAG_OK) return rc;
-  const int num_kb = dim / kBlockK;
-  using L = SearchLayout<16, 16, 7>;
-  auto kern = search_topk_kernel<16, 16, 7, false, true>;
-  const size_t smem = L::smem_bytes();
-  rc = ensure_smem_attr<KernelTag<16, 16, 7, false, true>>(kern, smem);
+  int rc = make_tmap_bf16_2d(&tm_corpus, corpus, uint64_t(n_rows), uint64_t(dim), uint64_t(row_stride) * 2, kTileRows);
   if (rc != CRAG_OK) return rc;
   for (int q0 = 0; q0 < nq; q0 += kNQ) {
     const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
     CUtensorMap tm_q;
-    rc = make_tmap_bf16_2d(&tm_q, static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, uint64_t(nqc), uint64_t(dim), uint64_t(dim) * 2, kNQ);
+    rc = make_query_tmap(&tm_q, queries, q0, nqc, dim);
     if (rc != CRAG_OK) return rc;
-    ScoreArgs sa{out_scores + int64_t(q0) * out_ld, out_ld, nullptr, nullptr, 0};
-    kern<<<grid, kSearchThreads, smem, stream>>>(tm_corpus, tm_q, int(n_rows), num_kb, nqc, 1, nullptr, nullptr, 0u, 0, nullptr,
-                                                 part_minmax, sa);
-    CRAG_CUDA_OK(cudaGetLastError());
+    ScoreArgs pass = sa;
+    if (sa.best_id) pass.base_id = q0;
+    else pass.out = sa.out + int64_t(q0) * sa.ld;
+    rc = launch_scan<16, 16, 7, false, true>(tm_corpus, tm_q, int(n_rows), dim / kBlockK, nqc, 1, grid, nullptr, nullptr, 0u, 0, nullptr, part_minmax, pass, stream);
+    if (rc != CRAG_OK) return rc;
     if (out_minmax) {
       minmax_reduce_kernel<<<nqc, 32, 0, stream>>>(part_minmax, grid, nqc, out_minmax + size_t(q0) * 2);
       CRAG_CUDA_OK(cudaGetLastError());
     }
   }
   return CRAG_OK;
+}
+}  // namespace
+}  // namespace crag
+
+extern "C" int crag_search_scores(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,
+                                  const void* queries, int nq, float* out_scores, int64_t out_ld, float* out_minmax,
+                                  void* workspace, size_t workspace_bytes, crag_stream_t stream) {
+  const SearchPlan plan = plan_search(1);
+  int rc = check_search_args(corpus, n_rows, dim, corpus_row_stride, queries, nq, 1, workspace, workspace_bytes, plan);
+  if (rc != CRAG_OK) return rc;
+  if (!out_scores || out_ld < n_rows) return fail(CRAG_ERR_INVALID, "crag_search_scores: need out_scores and out_ld >= n_rows");
+  return score_passes(corpus, n_rows, dim, corpus_row_stride, queries, nq, ScoreArgs{out_scores, out_ld, nullptr, nullptr, 0}, out_minmax, workspace,
+                      plan, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------ fused finalize + exchange (row-sharded index)
@@ -635,12 +634,11 @@ extern "C" int crag_search_finalize_exchange(const void* workspace, size_t works
   const uint64_t* part_keys = static_cast<const uint64_t*>(workspace);
   const float* part_minmax = reinterpret_cast<const float*>(static_cast<const uint8_t*>(workspace) + plan.keys_bytes);
   const int parts = scan_grid(n_rows, plan);
-  if (k <= 32)
-    finalize_exchange_kernel<32, 32><<<nq, 128, 0, stream>>>(part_keys, part_minmax, parts, nq, k, row_offset, peer_bufs, rank, world, epochs, status, out_ids, out_scores, out_minmax);
-  else if (k <= 64)
-    finalize_exchange_kernel<64, 64><<<nq, 128, 0, stream>>>(part_keys, part_minmax, parts, nq, k, row_offset, peer_bufs, rank, world, epochs, status, out_ids, out_scores, out_minmax);
-  else
-    finalize_exchange_kernel<128, 128><<<nq, 128, 0, stream>>>(part_keys, part_minmax, parts, nq, k, row_offset, peer_bufs, rank, world, epochs, status, out_ids, out_scores, out_minmax);
+  with_merge_tier(k, [&](auto tier) {   // one CTA per query
+    constexpr int T = decltype(tier)::value;
+    finalize_exchange_kernel<T, T><<<nq, 128, 0, stream>>>(part_keys, part_minmax, parts, nq, k, row_offset, peer_bufs, rank,
+                                                           world, epochs, status, out_ids, out_scores, out_minmax);
+  });
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }
@@ -651,34 +649,12 @@ extern "C" int crag_search_finalize_exchange(const void* workspace, size_t works
 // running best in (best_score, best_id).  Replaces a torch matmul + argmax over [rows, nlist] score blocks.
 extern "C" int crag_ivf_assign(const void* rows, int64_t n_rows, int dim, int64_t row_stride, const void* centroids,
                                int nlist, float* best_score, int32_t* best_id, void* workspace, size_t workspace_bytes,
-                               crag_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+                               crag_stream_t stream) {
   const SearchPlan plan = plan_search(1);
   int rc = check_search_args(rows, n_rows, dim, row_stride, centroids, nlist, 1, workspace, workspace_bytes, plan);
   if (rc != CRAG_OK) return rc;
   if (!best_score || !best_id) return fail(CRAG_ERR_INVALID, "crag_ivf_assign: null output pointer");
-  const int grid = scan_grid(n_rows, plan);
-  if (grid == 0) return CRAG_OK;
-  float* part_minmax = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + plan.keys_bytes);
-  CUtensorMap tm_rows;
-  rc = make_tmap_bf16_2d(&tm_rows, rows, uint64_t(n_rows), uint64_t(dim), uint64_t(row_stride) * 2, kTileRows);
-  if (rc != CRAG_OK) return rc;
-  const int num_kb = dim / kBlockK;
-  using L = SearchLayout<16, 16, 7>;
-  auto kern = search_topk_kernel<16, 16, 7, false, true>;
-  const size_t smem = L::smem_bytes();
-  rc = ensure_smem_attr<KernelTag<16, 16, 7, false, true>>(kern, smem);
-  if (rc != CRAG_OK) return rc;
   // the pass over centroid block 0 initialises every row's running best (-inf, list 0); later passes update it
-  for (int q0 = 0; q0 < nlist; q0 += kNQ) {
-    const int nqc = (nlist - q0) < kNQ ? (nlist - q0) : kNQ;
-    CUtensorMap tm_q;
-    rc = make_tmap_bf16_2d(&tm_q, static_cast<const uint8_t*>(centroids) + size_t(q0) * dim * 2, uint64_t(nqc), uint64_t(dim), uint64_t(dim) * 2, kNQ);
-    if (rc != CRAG_OK) return rc;
-    ScoreArgs sa{nullptr, 0, best_score, best_id, q0};
-    kern<<<grid, kSearchThreads, smem, stream>>>(tm_rows, tm_q, int(n_rows), num_kb, nqc, 1, nullptr, nullptr, 0u, 0, nullptr,
-                                                 part_minmax, sa);
-    CRAG_CUDA_OK(cudaGetLastError());
-  }
-  return CRAG_OK;
+  return score_passes(rows, n_rows, dim, row_stride, centroids, nlist, ScoreArgs{nullptr, 0, best_score, best_id, 0}, nullptr, workspace, plan,
+                      static_cast<cudaStream_t>(stream));
 }

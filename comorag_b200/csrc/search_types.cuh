@@ -1,5 +1,5 @@
-// Constants, shared-memory layout and argument structs of the shard scan kernel (search.cu), in a header of their own
-// so that tests/warp_emu can build the select warps' code (select_warps.inc.cuh) for the host.
+// Constants and argument structs of the shard scan kernel (search.cu), in a header of their own so that tests/warp_emu
+// can build the select warps (select_warps.cuh) for the host.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -28,29 +28,9 @@ constexpr int kProducerWarp = 8;
 // against 256 KB of corpus reads at dim 1024, so the scan stays HBM-bound.
 constexpr int kScoreTileBytes = kTileRows * kNQ * 4;  // 16 KB
 __host__ __device__ constexpr int score_slot(int row, int q) { return row * kNQ + (q ^ (row & 31)); }
-
-template <int KLIST, int CAP, int STAGES>
-struct SearchLayout {
-  static constexpr int kKeysPerQuery = KLIST + CAP;
-  // score-tile buffers: the scan may run this many tiles ahead of the select warps.  Together with STAGES they fill
-  // what the 227 KB of shared memory leave beside the candidate lists.
-  static constexpr int kAccStages = 4;
-  __host__ __device__ static constexpr size_t keys_bytes() { return size_t(kNQ) * kKeysPerQuery * 8; }
-  __host__ __device__ static constexpr size_t misc_bytes() {
-    return (2 * STAGES + 2 * kAccStages) * 8        // mbarriers
-           + kNQ * 8               // thr_key
-           + kNQ * 4               // thr_f
-           + kNQ * 4               // cnt
-           + kNQ * 8 + kNQ * 4     // continuation bound (key, score)
-           + kNQ * 8               // pooled admission floor (key)
-           + 4 * kNQ * 8           // per-warp partial floors of a refresh
-           + 4 * kNQ * 2 * 4       // min/max cross-warp reduction
-           + 16;
-  }
-  __host__ __device__ static constexpr size_t smem_bytes() {
-    return 1024 + size_t(STAGES) * kStageTotalBytes + size_t(kAccStages) * kScoreTileBytes + keys_bytes() + misc_bytes();
-  }
-};
+// score-tile buffers: the scan may run this many tiles ahead of the select warps.  Together with the pipeline stages
+// they fill what the 227 KB of shared memory leave beside the candidate lists.
+constexpr int kAccStages = 4;
 
 // IVF variant of the scan (BASELINE config 4; semantic: oracle/ivf_oracle.py): the shard holds bf16 RESIDUALS grouped
 // by coarse list, every list padded to whole 128-row tiles, and a pass touches only the tiles of probed lists.

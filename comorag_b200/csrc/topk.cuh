@@ -14,6 +14,7 @@
 // candidate buffer.  flush_query() bitonic-sorts the whole thing in registers
 // (32 lanes x EPL keys) and keeps the best k.
 #pragma once
+#include <math.h>
 #include <stdint.h>
 #include <cuda_runtime.h>
 
@@ -37,6 +38,15 @@ __device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int lane_mask) {
   lo = __shfl_xor_sync(0xffffffffu, lo, lane_mask);
   hi = __shfl_xor_sync(0xffffffffu, hi, lane_mask);
   return (static_cast<uint64_t>(hi) << 32) | lo;
+}
+
+// (min, max) of a warp's (a, b) pairs, left in every lane (xor butterfly, strides 16 .. 1)
+__device__ __forceinline__ void warp_minmax(float& a, float& b) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a = fminf(a, __shfl_xor_sync(0xffffffffu, a, o));
+    b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
+  }
 }
 
 // Bitonic sort, descending, of 32*EPL keys held EPL per lane in blocked order

@@ -1,13 +1,15 @@
-"""The SIMT parts of the kernels on the CPU.  csrc/topk.cuh, pool_floor.cuh, merge_kernels.cuh, rank_kernels.cuh and
-encoder_simt.cuh hold no wgmma / TMA / mbarrier code, so the SAME headers the library compiles are compiled for the
-host with CUDA threads as fibers (tests/warp_emu: warp collectives, __syncthreads, shared memory, one OS thread per
-rank with real atomics for the cross-rank exchange) and checked against plain C++ models:
+"""The SIMT parts of the kernels on the CPU.  csrc/topk.cuh, pool_floor.cuh, select_warps.cuh, merge_kernels.cuh,
+rank_kernels.cuh and encoder_simt.cuh hold no wgmma / TMA / mbarrier code, so the SAME headers the library compiles
+are compiled for the host with CUDA threads as fibers (tests/warp_emu: warp collectives, __syncthreads, named
+barriers, shared memory, one OS thread per rank with real atomics for the cross-rank exchange) and checked against
+plain C++ models:
   selector_emu_test.cpp  bitonic sort, flush / insert list maintenance, select_stream, and the pooled admission
                          floors -- above all the property exactness rests on: >= k published keys reach the floor
-  select_emu_test.cpp    the SELECT WARPS of the headline kernel (csrc/select_warps.inc.cuh, the text search_topk_kernel
-                         #includes): admission, warp-ballot compaction, flushes, pooled-floor refreshes across CTAs,
-                         drain, rank continuation, score-all and IVF variants -- fed a score matrix in place of
-                         the score-tile read, merged by the emulated merge kernel, compared bit for bit with the exact top-k
+  select_emu_test.cpp    the SELECT WARPS of the headline kernel (csrc/select_warps.cuh, the functions search_topk_kernel
+                         calls): admission, warp-ballot compaction, flushes, pooled-floor refreshes across CTAs,
+                         drain, rank continuation, score-all (and assignment) and IVF variants -- fed a score
+                         matrix as their score-tile source, merged by the emulated merge kernel, compared bit for bit
+                         with the exact top-k
   encoder_emu_test.cpp   embedding + LayerNorm, LayerNorm, masked mean pool + L2 normalise (K3) and the classifier
                          head (csrc/encoder_simt.cuh) against double-precision models
   kernel_emu_test.cpp    the IVF plan / id-map kernels, the radix-rank kernels (full permutation == stable descending
@@ -60,12 +62,14 @@ def test_selector_primitives_match_their_models_on_emulated_lanes(emu_binary):
 
 
 def test_the_emulated_headers_are_the_ones_the_kernel_includes():
-    """No copy of the selector lives under tests/: the emulation includes csrc/topk.cuh and csrc/pool_floor.cuh, and
-    search.cu includes the same two files."""
+    """No copy of the selector lives under tests/: the emulation includes csrc/topk.cuh, csrc/pool_floor.cuh and
+    csrc/select_warps.cuh, and search.cu includes the same files."""
     test_src = open(os.path.join(EMU, "selector_emu_test.cpp")).read()
     assert '#include "topk.cuh"' in test_src and '#include "pool_floor.cuh"' in test_src
     kernel_src = open(os.path.join(CSRC, "search.cu")).read()
     assert '#include "topk.cuh"' in kernel_src and '#include "pool_floor.cuh"' in kernel_src
+    assert '#include "select_warps.cuh"' in kernel_src
+    assert '#include "select_warps.cuh"' in open(os.path.join(EMU, "select_shell.h")).read()
     ktest_src = open(os.path.join(EMU, "kernel_emu_test.cpp")).read()
     assert '#include "merge_kernels.cuh"' in ktest_src and '#include "rank_kernels.cuh"' in ktest_src
     assert '#include "merge_kernels.cuh"' in kernel_src
@@ -152,27 +156,31 @@ def _build_select_test(csrc_dir, exe):
     return exe
 
 
-def test_select_warps_of_the_scan_kernel_on_emulated_blocks(tmp_path):
-    """search_topk_kernel's select warps -- the text the kernel itself #includes -- on adversarial score matrices
+def test_select_warps_header_of_the_scan_kernel_on_emulated_blocks(tmp_path):
+    """search_topk_kernel's select warps -- the functions the kernel itself calls -- on adversarial score matrices
     (ascending with the row id, all rows equal, three score levels, planted neighbours in the tail, random), k from 1
     to 128, 1 to 148 CTAs sharing the pooled floor -- run one after the other and all resident together in random
     interleavings --, with and without the tile permutation; rank continuation over
-    several pages; the score-all and IVF variants.  Ids, scores and (min, max) must equal the exact answer."""
+    several pages; the score-all variant and its assignment mode (running argmax over several centroid blocks, ties
+    across blocks); the IVF variant.  Ids, scores and (min, max) must equal the exact answer."""
     if shutil.which("g++") is None:
         pytest.skip("g++ not installed")
-    kernel_src = open(os.path.join(CSRC, "search.cu")).read()
-    assert kernel_src.count('#include "select_warps.inc.cuh"') == 3      # the kernel is built from the very same text
+    # the kernel and the emulation are built from the very same header
+    assert '#include "select_warps.cuh"' in open(os.path.join(CSRC, "search.cu")).read()
+    assert '#include "select_warps.cuh"' in open(os.path.join(EMU, "select_shell.h")).read()
+    assert not [f for f in os.listdir(CSRC) if f.endswith(".inc.cuh")], "kernel code pasted in as text"
     exe = _build_select_test(CSRC, tmp_path / "select_emu_test")
     r = subprocess.run([str(exe), "1"], capture_output=True, text=True, timeout=1800)
     assert r.returncode == 0, r.stdout + r.stderr
     assert r.stdout.strip().endswith("ALL OK")
     for group in ("select warps <64, 64>: all rows equal", "select warps <128, 128>: planted neighbours in the last rows, 75699 rows on 148 CTAs",
                   "select warps <128, 128>: all rows equal, 75699 rows on 148 CTAs (4 tiles each), nq = 32, k = 100, pool on, permutation on, CTAs interleaved",
-                  "rank continuation <128, 128>: random", "IVF variant <128, 128>: 64 lists", "score-all variant: 4475 rows"):
+                  "rank continuation <128, 128>: random", "IVF variant <128, 128>: 64 lists", "score-all variant: 4475 rows",
+                  "assign mode: 1525 rows on 3 CTAs, 103 centroids in 4 blocks"):
         assert f"ok  {group}" in r.stdout, group
 
 
-def test_emulation_catches_a_selector_that_drops_a_tie(tmp_path):
+def test_emulation_catches_an_admission_test_that_drops_a_tie(tmp_path):
     """Mutation check: an admission test that compares scores only (strictly) loses rows that tie the k-th score with a
     smaller row id -- the all-equal / few-levels corpora and the continuation pages must expose it."""
     if shutil.which("g++") is None:
@@ -182,10 +190,10 @@ def test_emulation_catches_a_selector_that_drops_a_tie(tmp_path):
     for h in os.listdir(CSRC):
         if h.endswith(".cuh"):
             shutil.copy(os.path.join(CSRC, h), mutated / h)
-    src = (mutated / "select_warps.inc.cuh").read_text()
-    needle = "if (s >= thr_f[q] && s <= bnd_f[q] && make_key(s, uint32_t(row)) > thr_key[q]) pending |= 1u << q;"
-    assert src.count(needle) == 2          # flat and IVF admission
-    (mutated / "select_warps.inc.cuh").write_text(src.replace(needle, "if (s > thr_f[q] && s <= bnd_f[q]) pending |= 1u << q;"))
+    src = (mutated / "select_warps.cuh").read_text()
+    needle = "return s >= thr_f[q] && s <= bnd_f[q] && make_key(s, row) > thr_key[q];"
+    assert src.count(needle) == 1          # the one admission test of the flat and IVF scans
+    (mutated / "select_warps.cuh").write_text(src.replace(needle, "return s > thr_f[q] && s <= bnd_f[q];"))
     exe = _build_select_test(mutated, tmp_path / "mutant")
     r = subprocess.run([str(exe), "ties"], capture_output=True, text=True, timeout=1800)
     assert r.returncode != 0 and "FAILED" in r.stderr

@@ -13,7 +13,7 @@
 
 using namespace crag;
 
-template <int KLIST, int CAP, int STAGES>
+template <int KLIST, int CAP>
 static void census(int64_t rows, int k, int nq, int grid, bool concurrent) {
   std::mt19937_64 rng(5);
   std::normal_distribution<float> nd(0.f, 0.03125f);     // q . x of unit vectors at dim 1024
@@ -21,16 +21,16 @@ static void census(int64_t rows, int k, int nq, int grid, bool concurrent) {
   for (auto& v : scores) v = nd(rng);
   std::vector<uint64_t> part_keys(size_t(grid) * kNQ * k), pool(size_t(grid) * kPoolSlots * kNQ, 0ull);
   std::vector<float> part_mm(size_t(grid) * kNQ * 2);
-  g_src = ScoreSource{scores.data(), rows, nullptr};
+  g_src = MatrixScoreTiles{scores.data(), rows, nullptr};
   const int64_t tiles = (rows + kTileRows - 1) / kTileRows;
   const int shift = 3;
   const uint32_t perm = perm_multiplier(tiles >> shift);
   warp_emu::census() = warp_emu::Census{};
   auto scan = [&] {
-    search_select_shell<KLIST, CAP, STAGES>(int(rows), nq, k, nullptr, pool.data(), perm, shift, part_keys.data(), part_mm.data(), NoIvfArgs{});
+    search_select_shell<KLIST, CAP>(int(rows), nq, k, nullptr, pool.data(), perm, shift, part_keys.data(), part_mm.data(), NoIvfArgs{});
   };
-  if (concurrent) warp_emu::launch_concurrent(grid, kSearchThreads, scan, select_shell_smem_bytes<KLIST, CAP>(), 7);
-  else warp_emu::launch(grid, kSearchThreads, scan, select_shell_smem_bytes<KLIST, CAP>());
+  if (concurrent) warp_emu::launch_concurrent(grid, kSearchThreads, scan, SelectSmem<KLIST, CAP>::bytes(), 7);
+  else warp_emu::launch(grid, kSearchThreads, scan, SelectSmem<KLIST, CAP>::bytes());
   const warp_emu::Census c = warp_emu::census();
   const double warps = double(grid) * 4.0, lanes = warps * 32.0;
   const double tiles_per_cta = double(tiles) / grid;
@@ -49,7 +49,7 @@ int main(int argc, char** argv) {
   const int k = argc > 2 ? atoi(argv[2]) : 100;
   const int nq = argc > 3 ? atoi(argv[3]) : 32;
   const bool concurrent = argc > 4 && atoi(argv[4]) != 0;     // all 148 CTAs resident together, as on the GPU
-  if (k <= 64) census<64, 64, 7>(rows, k, nq, 148, concurrent);
-  else census<128, 128, 5>(rows, k, nq, 148, concurrent);
+  if (k <= 64) census<64, 64>(rows, k, nq, 148, concurrent);
+  else census<128, 128>(rows, k, nq, 148, concurrent);
   return 0;
 }

@@ -1,14 +1,13 @@
-// The select warps of the shard-scan kernel on the CPU.  csrc/select_warps.inc.cuh is the TEXT of search_topk_kernel's
-// select-warp code (the kernel #includes it, its SASS is unchanged); here the same three sections are included inside
-// a host function whose locals carry the names the kernel's have, with
-//   score-tile read       -> a score matrix this test supplies (the selection logic does not care where scores come
+// The select warps of the shard-scan kernel on the CPU.  select_shell.h calls the kernel's own select_warps() and
+// SelectSmem (csrc/select_warps.cuh) with
+//   score-tile source     -> a score matrix this test supplies (the selection logic does not care where scores come
 //                            from: any fp32 matrix is a valid "q . x" for it, ties and adversarial orders included)
-//   mbarrier waits        -> nothing (a tile is "there" when it is asked for)
 //   named barriers        -> the fiber emulator's (warp_emu.h)
 // so that everything the four select warps do runs for real: the per-row admission test against thr_f / thr_key / the
 // continuation bound, the warp-ballot compaction into the candidate buffers, flushes, the pooled-floor publishes and
 // refreshes across CTAs, the first-tile fast path, the tail drain, the per-CTA lists and (min, max); also the rank
-// continuation (k > 128), the score-all variant and the IVF variant (with the emulated plan kernel in front).  The per-CTA
+// continuation (k > 128), the score-all variant with its assignment mode, and the IVF variant (with the emulated plan
+// kernel in front).  The per-CTA
 // lists then go through the emulated merge_topk_kernel and the answer is compared, bit for bit, with the exact top-k
 // of the score matrix under the engine's rule (score descending, row ascending).
 #include <algorithm>
@@ -74,17 +73,17 @@ static std::vector<uint64_t> exact_keys(const std::vector<float>& s, int64_t row
 static uint64_t g_concurrent_seed = 0;
 
 // one pass = crag_search_scan + crag_search_finalize: scan shell on `grid` blocks, then the emulated merge kernel
-template <int KLIST, int CAP, int STAGES>
+template <int KLIST, int CAP>
 static void run_pass(const std::vector<float>& scores, int64_t rows, int grid, int nq, int k, bool use_pool, uint32_t perm_mul, int perm_shift,
                      const uint64_t* after, std::vector<int64_t>& ids, std::vector<float>& sc, std::vector<float>& mm, std::vector<uint64_t>& last) {
   std::vector<uint64_t> part_keys(size_t(grid) * kNQ * k, 0xDEADull), pool(size_t(grid) * kPoolSlots * kNQ, 0ull);
   std::vector<float> part_mm(size_t(grid) * kNQ * 2, -5.f);
-  g_src = ScoreSource{scores.data(), rows, nullptr};
+  g_src = MatrixScoreTiles{scores.data(), rows, nullptr};
   auto scan = [&] {
-    search_select_shell<KLIST, CAP, STAGES>(int(rows), nq, k, after, use_pool ? pool.data() : nullptr, perm_mul, perm_shift, part_keys.data(), part_mm.data(), NoIvfArgs{});
+    search_select_shell<KLIST, CAP>(int(rows), nq, k, after, use_pool ? pool.data() : nullptr, perm_mul, perm_shift, part_keys.data(), part_mm.data(), NoIvfArgs{});
   };
-  if (g_concurrent_seed) warp_emu::launch_concurrent(grid, kSearchThreads, scan, select_shell_smem_bytes<KLIST, CAP>(), g_concurrent_seed);
-  else warp_emu::launch(grid, kSearchThreads, scan, select_shell_smem_bytes<KLIST, CAP>());
+  if (g_concurrent_seed) warp_emu::launch_concurrent(grid, kSearchThreads, scan, SelectSmem<KLIST, CAP>::bytes(), g_concurrent_seed);
+  else warp_emu::launch(grid, kSearchThreads, scan, SelectSmem<KLIST, CAP>::bytes());
   ids.assign(size_t(nq) * k, -5); sc.assign(size_t(nq) * k, -5.f); mm.assign(size_t(nq) * 2, -5.f); last.assign(nq, 1);
   warp_emu::launch(nq, 128, [&] {
     merge_topk_kernel<KLIST, CAP, false>(part_keys.data(), nullptr, nullptr, part_mm.data(), grid, kNQ, nq, k, 1000, 0, 0, 0, ids.data(), sc.data(), mm.data(), last.data());
@@ -93,7 +92,7 @@ static void run_pass(const std::vector<float>& scores, int64_t rows, int grid, i
 
 constexpr uint32_t kAutoPerm = 0xFFFFFFFFu;     // "ask perm_multiplier()", as the library's host code does
 
-template <int KLIST, int CAP, int STAGES>
+template <int KLIST, int CAP>
 static void test_topk(Data d, int grid, int tiles_per_cta, int ragged, int nq, int k, bool use_pool, uint32_t perm_mul, int perm_shift) {
   const int64_t rows = int64_t(grid) * tiles_per_cta * kTileRows - ragged;
   const int64_t n_tiles = (rows + kTileRows - 1) / kTileRows;
@@ -107,7 +106,7 @@ static void test_topk(Data d, int grid, int tiles_per_cta, int ragged, int nq, i
   std::vector<int64_t> ids;
   std::vector<float> sc, mm;
   std::vector<uint64_t> last;
-  run_pass<KLIST, CAP, STAGES>(scores, rows, grid, nq, k, use_pool, perm_mul, perm_shift, nullptr, ids, sc, mm, last);
+  run_pass<KLIST, CAP>(scores, rows, grid, nq, k, use_pool, perm_mul, perm_shift, nullptr, ids, sc, mm, last);
   for (int q = 0; q < nq; ++q) {
     std::vector<uint64_t> want = exact_keys(scores, rows, q);
     for (int j = 0; j < k; ++j) {
@@ -125,7 +124,7 @@ static void test_topk(Data d, int grid, int tiles_per_cta, int ragged, int nq, i
 }
 
 // rank continuation (crag_search_topk_after): pages of k ranks, each admitting only keys below the previous page's last
-template <int KLIST, int CAP, int STAGES>
+template <int KLIST, int CAP>
 static void test_continuation(Data d, int grid, int tiles_per_cta, int nq, int k, int pages) {
   const int64_t rows = int64_t(grid) * tiles_per_cta * kTileRows - 17;
   std::vector<float> scores = make_scores(rows, d);
@@ -134,7 +133,7 @@ static void test_continuation(Data d, int grid, int tiles_per_cta, int nq, int k
     std::vector<int64_t> ids;
     std::vector<float> sc, mm;
     std::vector<uint64_t> last;
-    run_pass<KLIST, CAP, STAGES>(scores, rows, grid, nq, k, true, perm_multiplier(((rows + kTileRows - 1) / kTileRows) >> 1), 1,
+    run_pass<KLIST, CAP>(scores, rows, grid, nq, k, true, perm_multiplier(((rows + kTileRows - 1) / kTileRows) >> 1), 1,
                                  page ? after.data() : nullptr, ids, sc, mm, last);
     for (int q = 0; q < nq; ++q) {
       std::vector<uint64_t> want = exact_keys(scores, rows, q);
@@ -155,10 +154,10 @@ static void test_score_all(int grid, int tiles_per_cta, int nq) {
   const int64_t rows = int64_t(grid) * tiles_per_cta * kTileRows - 5;
   std::vector<float> scores = make_scores(rows, Data::Random);
   std::vector<float> out(size_t(nq) * rows, -7.f), part_mm(size_t(grid) * kNQ * 2, -5.f);
-  g_src = ScoreSource{scores.data(), rows, nullptr};
+  g_src = MatrixScoreTiles{scores.data(), rows, nullptr};
   warp_emu::launch(grid, kSearchThreads, [&] {
-    search_select_shell<16, 16, 9, false, true>(int(rows), nq, 1, nullptr, nullptr, 0u, 0, nullptr, part_mm.data(), ScoreArgs{out.data(), rows, nullptr, nullptr, 0});
-  }, select_shell_smem_bytes<16, 16>());
+    search_select_shell<16, 16, false, true>(int(rows), nq, 1, nullptr, nullptr, 0u, 0, nullptr, part_mm.data(), ScoreArgs{out.data(), rows, nullptr, nullptr, 0});
+  }, SelectSmem<16, 16>::bytes());
   for (int q = 0; q < nq; ++q) {
     float mn = INFINITY, mx = -INFINITY;
     for (int64_t r = 0; r < rows; ++r) {
@@ -172,11 +171,45 @@ static void test_score_all(int grid, int tiles_per_cta, int nq) {
   printf("ok  score-all variant: %lld rows on %d CTAs, nq = %d: every score stored, (min, max) exact\n", (long long)rows, grid, nq);
 }
 
+// assignment mode (crag_ivf_assign): one score-all pass per block of 32 centroids, each row keeping its running argmax;
+// three score levels, so most rows tie their best score across blocks -- the smallest centroid id must win
+static void test_assign(int grid, int tiles_per_cta, int nlist) {
+  const int64_t rows = int64_t(grid) * tiles_per_cta * kTileRows - 11;
+  std::vector<float> all(size_t(rows) * nlist);
+  for (auto& v : all) v = float(int(rng() % 3)) * 0.1f;
+  std::vector<float> best_score(rows, -7.f), part_mm(size_t(grid) * kNQ * 2, -5.f);
+  std::vector<int32_t> best_id(rows, -7);
+  for (int q0 = 0; q0 < nlist; q0 += kNQ) {
+    const int nqc = std::min(kNQ, nlist - q0);
+    std::vector<float> block(size_t(rows) * kNQ, 0.f);
+    for (int64_t r = 0; r < rows; ++r)
+      for (int q = 0; q < nqc; ++q) block[size_t(r) * kNQ + q] = all[size_t(r) * nlist + q0 + q];
+    g_src = MatrixScoreTiles{block.data(), rows, nullptr};
+    warp_emu::launch(grid, kSearchThreads, [&] {
+      search_select_shell<16, 16, false, true>(int(rows), nqc, 1, nullptr, nullptr, 0u, 0, nullptr, part_mm.data(),
+                                               ScoreArgs{nullptr, 0, best_score.data(), best_id.data(), q0});
+    }, SelectSmem<16, 16>::bytes());
+  }
+  int64_t tied_across_blocks = 0;
+  for (int64_t r = 0; r < rows; ++r) {
+    int want = 0;
+    for (int c = 1; c < nlist; ++c)
+      if (all[size_t(r) * nlist + c] > all[size_t(r) * nlist + want]) want = c;
+    const float ws = all[size_t(r) * nlist + want];
+    for (int c = kNQ; c < nlist; ++c) tied_across_blocks += (want < kNQ && all[size_t(r) * nlist + c] == ws) ? 1 : 0;
+    REQUIRE(best_id[r] == want && __float_as_uint(best_score[r]) == __float_as_uint(ws),
+            "assign: row %lld holds centroid %d (%g), want %d (%g)", (long long)r, best_id[r], best_score[r], want, ws);
+  }
+  REQUIRE(tied_across_blocks > 0, "test bug: no row ties its best score across centroid blocks");
+  printf("ok  assign mode: %lld rows on %d CTAs, %d centroids in %d blocks: running argmax exact, ties to the smaller id\n",
+         (long long)rows, grid, nlist, (nlist + kNQ - 1) / kNQ);
+}
+
 // IVF variant (crag_ivf_search): the plan kernel builds query masks / coarse terms / the work-list, the select warps walk
 // the work-list, add the coarse term and skip the queries that do not probe the tile's list; model = oracle/ivf_oracle.py
 // restated over the given residual scores: candidates of query q = the real rows of the lists it probes, score =
 // residual score + coarse score (fp32, in that order), best k by (score desc, stored row asc)
-template <int KLIST, int CAP, int STAGES>
+template <int KLIST, int CAP>
 static void test_ivf(int nlist, int nprobe, int grid, int nq, int k) {
   std::vector<int32_t> list_rows(nlist), tile_start(nlist + 1, 0);
   for (int l = 0; l < nlist; ++l) {
@@ -202,11 +235,11 @@ static void test_ivf(int nlist, int nprobe, int grid, int nq, int k) {
   });
   std::vector<uint64_t> part_keys(size_t(grid) * kNQ * k, 0xDEADull), pool(size_t(grid) * kPoolSlots * kNQ, 0ull);
   std::vector<float> part_mm(size_t(grid) * kNQ * 2, -5.f);
-  g_src = ScoreSource{resid.data(), stored, work.data()};
+  g_src = MatrixScoreTiles{resid.data(), stored, work.data()};
   const IvfArgs args{work.data(), &n_work, mask.data(), coarse.data()};
   warp_emu::launch(grid, kSearchThreads, [&] {
-    search_select_shell<KLIST, CAP, STAGES, true, false>(0, nq, k, nullptr, pool.data(), 0u, 0, part_keys.data(), part_mm.data(), args);
-  }, select_shell_smem_bytes<KLIST, CAP>());
+    search_select_shell<KLIST, CAP, true, false>(0, nq, k, nullptr, pool.data(), 0u, 0, part_keys.data(), part_mm.data(), args);
+  }, SelectSmem<KLIST, CAP>::bytes());
   std::vector<int64_t> ids(size_t(nq) * k, -5);
   std::vector<float> sc(size_t(nq) * k, -5.f), mm(size_t(nq) * 2, -5.f);
   warp_emu::launch(nq, 128, [&] {
@@ -239,10 +272,10 @@ static void test_ivf(int nlist, int nprobe, int grid, int nq, int k) {
 
 int main(int argc, char** argv) {
   if (argc > 1 && std::string(argv[1]) == "ties") {     // the tie-heavy cases only (what the mutation tests run)
-    test_topk<64, 64, 7>(Data::AllEqual, 4, 8, 33, 32, 10, true, 37u, 3);
-    test_topk<64, 64, 7>(Data::FewLevels, 4, 8, 33, 32, 10, true, 37u, 3);
-    test_continuation<128, 128, 5>(Data::FewLevels, 4, 6, 32, 128, 3);
-    test_continuation<64, 64, 7>(Data::AllEqual, 3, 4, 3, 50, 5);
+    test_topk<64, 64>(Data::AllEqual, 4, 8, 33, 32, 10, true, 37u, 3);
+    test_topk<64, 64>(Data::FewLevels, 4, 8, 33, 32, 10, true, 37u, 3);
+    test_continuation<128, 128>(Data::FewLevels, 4, 6, 32, 128, 3);
+    test_continuation<64, 64>(Data::AllEqual, 3, 4, 3, 50, 5);
     printf("ALL OK\n");
     return 0;
   }
@@ -256,16 +289,16 @@ int main(int argc, char** argv) {
       const int ragged = int(rng() % 128), nq = (rng() % 3 == 0) ? 1 + int(rng() % 32) : 32;
       // kAutoPerm: the multiplier search.cu's perm_multiplier() picks for the drawn shape (it must be coprime to the
       // number of tile groups -- an arbitrary constant would visit some tiles twice and others never)
-      if (regime == 0) test_topk<64, 64, 7>(d, 2 + int(rng() % 10), 3 + int(rng() % 20), ragged, nq, 1 + int(rng() % 16), true, kAutoPerm, int(rng() % 4));
-      else if (regime == 1) test_topk<64, 64, 7>(d, 20 + int(rng() % 60), 3 + int(rng() % 6), ragged, nq, 17 + int(rng() % 48), true, kAutoPerm, int(rng() % 3));
-      else if (regime == 2) test_topk<128, 128, 5>(d, 130 + int(rng() % 30), 3 + int(rng() % 3), ragged, nq, 65 + int(rng() % 40), true, kAutoPerm, 1);
-      else if (regime == 3) test_topk<128, 128, 5>(d, 4 + int(rng() % 12), 4 + int(rng() % 12), ragged, nq, 100 + int(rng() % 29), true, kAutoPerm, int(rng() % 3));
+      if (regime == 0) test_topk<64, 64>(d, 2 + int(rng() % 10), 3 + int(rng() % 20), ragged, nq, 1 + int(rng() % 16), true, kAutoPerm, int(rng() % 4));
+      else if (regime == 1) test_topk<64, 64>(d, 20 + int(rng() % 60), 3 + int(rng() % 6), ragged, nq, 17 + int(rng() % 48), true, kAutoPerm, int(rng() % 3));
+      else if (regime == 2) test_topk<128, 128>(d, 130 + int(rng() % 30), 3 + int(rng() % 3), ragged, nq, 65 + int(rng() % 40), true, kAutoPerm, 1);
+      else if (regime == 3) test_topk<128, 128>(d, 4 + int(rng() % 12), 4 + int(rng() % 12), ragged, nq, 100 + int(rng() % 29), true, kAutoPerm, int(rng() % 3));
       else if (regime == 4) {
-        if (rng() % 2) test_continuation<128, 128, 5>(d, 2 + int(rng() % 6), 2 + int(rng() % 8), nq, 65 + int(rng() % 64), 2 + int(rng() % 3));
-        else test_continuation<64, 64, 7>(d, 2 + int(rng() % 6), 2 + int(rng() % 8), nq, 1 + int(rng() % 64), 2 + int(rng() % 4));
+        if (rng() % 2) test_continuation<128, 128>(d, 2 + int(rng() % 6), 2 + int(rng() % 8), nq, 65 + int(rng() % 64), 2 + int(rng() % 3));
+        else test_continuation<64, 64>(d, 2 + int(rng() % 6), 2 + int(rng() % 8), nq, 1 + int(rng() % 64), 2 + int(rng() % 4));
       } else {
-        if (rng() % 2) test_ivf<128, 128, 5>(8 + int(rng() % 200), 1 + int(rng() % 8), 1 + int(rng() % 9), nq, 65 + int(rng() % 64));
-        else test_ivf<64, 64, 7>(8 + int(rng() % 200), 1 + int(rng() % 8), 1 + int(rng() % 9), nq, 1 + int(rng() % 64));
+        if (rng() % 2) test_ivf<128, 128>(8 + int(rng() % 200), 1 + int(rng() % 8), 1 + int(rng() % 9), nq, 65 + int(rng() % 64));
+        else test_ivf<64, 64>(8 + int(rng() % 200), 1 + int(rng() % 8), 1 + int(rng() % 9), nq, 1 + int(rng() % 64));
       }
     }
     printf("ALL OK\n");
@@ -274,32 +307,33 @@ int main(int argc, char** argv) {
   const int scale = argc > 1 ? atoi(argv[1]) : 1;
   // the headline regime: k = 10, long scans (refresh schedule 2 / 12 / 48 / 128), every data set
   for (Data d : {Data::Random, Data::Ascending, Data::AllEqual, Data::FewLevels, Data::PlantedTail})
-    test_topk<64, 64, 7>(d, 4, 50 * scale, 33, 32, 10, true, 37u, 3);
-  test_topk<64, 64, 7>(Data::Random, 3, 132, 0, 32, 10, true, 0u, 0);          // no permutation; refresh at tile 128
-  test_topk<64, 64, 7>(Data::Random, 3, 5, 100, 7, 64, false, 0u, 0);          // no pool (short scans), nq < 32, k = KLIST
-  test_topk<64, 64, 7>(Data::FewLevels, 5, 9, 1, 1, 1, true, 3u, 1);           // k = 1, one query
+    test_topk<64, 64>(d, 4, 50 * scale, 33, 32, 10, true, 37u, 3);
+  test_topk<64, 64>(Data::Random, 3, 132, 0, 32, 10, true, 0u, 0);          // no permutation; refresh at tile 128
+  test_topk<64, 64>(Data::Random, 3, 5, 100, 7, 64, false, 0u, 0);          // no pool (short scans), nq < 32, k = KLIST
+  test_topk<64, 64>(Data::FewLevels, 5, 9, 1, 1, 1, true, 3u, 1);           // k = 1, one query
   // config 4's regime: k = 100 on the 128-key selector, batch-of-8 bisection floor (k <= 0.8 x CTAs) on 148 CTAs
-  test_topk<128, 128, 5>(Data::Random, 148, 4, 77, 32, 100, true, 11u, 1);
-  test_topk<128, 128, 5>(Data::Ascending, 40, 10, 0, 32, 32, true, 7u, 2);     // 16 < k <= 0.8 x 40 CTAs
+  test_topk<128, 128>(Data::Random, 148, 4, 77, 32, 100, true, 11u, 1);
+  test_topk<128, 128>(Data::Ascending, 40, 10, 0, 32, 32, true, 7u, 2);     // 16 < k <= 0.8 x 40 CTAs
   // k > 0.8 x CTAs: all four keys per CTA pooled (pooled_kth_key), k = 128
-  test_topk<128, 128, 5>(Data::Ascending, 8, 20, 5, 32, 128, true, 3u, 2);
-  test_topk<128, 128, 5>(Data::Random, 2, 1, 100, 32, 100, false, 0u, 0);       // fewer rows than k per CTA list: -1 padding
+  test_topk<128, 128>(Data::Ascending, 8, 20, 5, 32, 128, true, 3u, 2);
+  test_topk<128, 128>(Data::Random, 2, 1, 100, 32, 100, false, 0u, 0);       // fewer rows than k per CTA list: -1 padding
   // the same regimes with all CTAs resident together, in two random interleavings each
   for (uint64_t seed : {11ull, 12ull}) {
     g_concurrent_seed = seed;
-    test_topk<64, 64, 7>(seed == 11 ? Data::Random : Data::FewLevels, 6, 30, 9, 32, 10, true, 37u, 3);
-    test_topk<128, 128, 5>(seed == 11 ? Data::AllEqual : Data::PlantedTail, 148, 4, 77, 32, 100, true, 11u, 1);
-    test_topk<128, 128, 5>(seed == 11 ? Data::FewLevels : Data::Random, 8, 20, 5, 32, 128, true, 3u, 2);
+    test_topk<64, 64>(seed == 11 ? Data::Random : Data::FewLevels, 6, 30, 9, 32, 10, true, 37u, 3);
+    test_topk<128, 128>(seed == 11 ? Data::AllEqual : Data::PlantedTail, 148, 4, 77, 32, 100, true, 11u, 1);
+    test_topk<128, 128>(seed == 11 ? Data::FewLevels : Data::Random, 8, 20, 5, 32, 128, true, 3u, 2);
   }
   g_concurrent_seed = 0;
-  test_continuation<128, 128, 5>(Data::Random, 4, 12, 5, 128, 4);
-  test_continuation<128, 128, 5>(Data::FewLevels, 4, 6, 32, 128, 3);
-  test_continuation<64, 64, 7>(Data::AllEqual, 3, 4, 3, 50, 5);
-  test_ivf<128, 128, 5>(64, 8, 5, 32, 100);
-  test_ivf<64, 64, 7>(200, 16, 7, 9, 10);
-  test_ivf<128, 128, 5>(12, 12, 3, 32, 128);      // nprobe = nlist: exact search over every list
+  test_continuation<128, 128>(Data::Random, 4, 12, 5, 128, 4);
+  test_continuation<128, 128>(Data::FewLevels, 4, 6, 32, 128, 3);
+  test_continuation<64, 64>(Data::AllEqual, 3, 4, 3, 50, 5);
+  test_ivf<128, 128>(64, 8, 5, 32, 100);
+  test_ivf<64, 64>(200, 16, 7, 9, 10);
+  test_ivf<128, 128>(12, 12, 3, 32, 128);      // nprobe = nlist: exact search over every list
   test_score_all(5, 7, 32);
   test_score_all(2, 3, 9);
+  test_assign(3, 4, 103);
   printf("ALL OK\n");
   return 0;
 }

@@ -39,6 +39,9 @@ static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }   // the GPU's r
 #define CRAG_DYNAMIC_SHARED(type, name) type* name = static_cast<type*>(warp_emu::dynamic_shared())
 namespace crag {
 static inline void bar_sync_group0_128() { warp_emu::named_barrier(1, 128); }
+// csrc/select_warps.cuh: the select warps' named barriers
+static inline void named_bar_sync(uint32_t id, uint32_t n) { warp_emu::named_barrier(int(id), int(n)); }
+static inline bool named_bar_or(uint32_t id, uint32_t n, bool p) { return warp_emu::named_barrier_or(int(id), int(n), p); }
 }  // namespace crag
 
 static inline uint32_t __float_as_uint(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
