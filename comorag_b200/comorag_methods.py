@@ -11,6 +11,11 @@ Each function keeps the reference method's name, signature, return type and side
 
 `retrieve_knn` (utils/embed_utils.py:8-97, called at ComoRAG.py:678) is a module-level name and is rebound by
 install() like the other imported names (comorag_b200.retrieval.retrieve_knn).
+
+GRAPH_METHODS, rebound only by install(graph=True), move the graph branch of tri_retrieve onto the device:
+
+    graph_search_with_fact_entities(self, query, link_top_k, ...)    ComoRAG.py:992-1055 (+ get_top_k_weights, :972-990)
+    run_ppr(self, reset_prob, damping=0.5)                           ComoRAG.py:1086-1105
 """
 from __future__ import annotations
 
@@ -18,9 +23,13 @@ import logging
 from typing import Dict, List, Tuple
 
 import numpy as np
+import torch
 
 from . import retrieval
 from .coalescer import BatcherClosed
+from .embedding_store import compute_mdhash_id
+from .graph import DeviceGraph
+from .index import rank_scores
 
 logger = logging.getLogger(__name__)
 
@@ -295,4 +304,121 @@ METHODS = {
     "get_query_embeddings": get_query_embeddings,
     "get_fact_scores": get_fact_scores,
     "dense_passage_retrieval": dense_passage_retrieval,
+}
+
+
+# ------------------------------------------------------------------------------------------------ graph search
+_graph_lock = __import__("threading").Lock()
+
+
+def _device_graph(self) -> DeviceGraph:
+    """self.graph as a DeviceGraph, built on first use and cached on the instance, keyed by (vcount, ecount): the
+    reference only ever adds vertices and edges (ComoRAG.py:779-841), so a changed graph changes one of the two."""
+    key = (self.graph.vcount(), self.graph.ecount())
+    cached = getattr(self, "_crag_graph", None)
+    if cached is None or cached[0] != key:
+        with _graph_lock:               # up to 16 tri_retrieve threads reach the first graph search together
+            cached = getattr(self, "_crag_graph", None)
+            if cached is None or cached[0] != key:
+                cached = (key, DeviceGraph.from_igraph(self.graph))
+                self._crag_graph = cached
+    return cached[1]
+
+
+def _passage_vertices(self) -> np.ndarray:
+    """self.passage_node_idxs as int64 (prepare_retrieval_objects assigns a new list when it rebuilds them)."""
+    idxs = self.passage_node_idxs
+    cached = getattr(self, "_crag_passage_vertices", None)
+    if cached is None or cached[0] is not idxs or len(cached[1]) != len(idxs):
+        cached = (idxs, np.asarray(idxs, dtype=np.int64).reshape(-1), {})
+        self._crag_passage_vertices = cached
+    return cached[1]
+
+
+def _passage_vertices_on(self, graph: DeviceGraph) -> torch.Tensor:
+    _passage_vertices(self)
+    on_device = self._crag_passage_vertices[2]
+    if graph.device not in on_device:
+        on_device[graph.device] = torch.as_tensor(self._crag_passage_vertices[1], device=graph.device)
+    return on_device[graph.device]
+
+
+def run_ppr(self, reset_prob: np.ndarray, damping: float = 0.5) -> Tuple[np.ndarray, np.ndarray]:
+    """ComoRAG.py:1086-1105: PPR over self.graph with run_ppr's reset sanitising, on the device (crag_ppr), then the
+    passages ranked by score on the device (crag_rank_scores).  Returns (sorted_doc_ids int64, sorted_doc_scores
+    float64) over self.passage_node_idxs; equal scores rank by ascending row."""
+    if damping is None:
+        damping = 0.5
+    graph = _device_graph(self)
+    scores = graph.personalized_pagerank(np.asarray(reset_prob, dtype=np.float64), damping,
+                                         vertices=_passage_vertices_on(self, graph))
+    ids, sorted_scores = rank_scores(scores)
+    return ids.cpu().numpy(), sorted_scores.cpu().numpy().astype(np.float64)
+
+
+def graph_search_with_fact_entities(self, query: str, link_top_k: int, query_fact_scores: np.ndarray,
+                                    top_k_facts: List[Tuple], top_k_fact_indices: List[str],
+                                    passage_node_weight: float = 0.05):
+    """ComoRAG.py:992-1055 with get_top_k_weights (:972-990): the same node weights, bit for bit, the same
+    used_phrases_with_scores and assertions, in O(facts + link_top_k) Python plus vectorised numpy:
+      * phrase weights live in a dict {vertex: weight} until the end; "zero every vertex outside the top-k phrase
+        keys" keeps exactly the entries whose key is among them;
+      * the passage weights are one scatter of min_max_normalize(dpr scores) * passage_node_weight;
+      * the per-passage linking_score_map entries (a get_row per passage) are not built: the map is local and never
+        returned, so nothing observable changes."""
+    linking_score_map = {}
+    phrase_scores = {}
+    phrase_weights = {}             # vertex -> weight: the nonzero-capable entries of the reference's dense array
+    phrase_keys = {}                # vertex -> its name (phrase key)
+    used_phrases_with_scores = {}
+    n_vertices = self.graph.vcount()
+
+    for rank, f in enumerate(top_k_facts):
+        subject_phrase = f[0].lower()
+        object_phrase = f[2].lower()
+        fact_score = query_fact_scores[top_k_fact_indices[rank]] if query_fact_scores.ndim > 0 else query_fact_scores
+        for phrase in [subject_phrase, object_phrase]:
+            phrase_key = compute_mdhash_id(content=phrase, prefix="entity-")
+            phrase_id = self.node_name_to_vertex_idx.get(phrase_key, None)
+            if phrase_id is not None:
+                w = np.float64(fact_score)
+                if self.ent_node_to_num_chunk[phrase_key] != 0:
+                    w /= self.ent_node_to_num_chunk[phrase_key]
+                phrase_weights[phrase_id] = w
+                phrase_keys[phrase_id] = phrase_key
+                if w > 0:
+                    used_phrases_with_scores[phrase] = w
+            if phrase not in phrase_scores:
+                phrase_scores[phrase] = []
+            phrase_scores[phrase].append(fact_score)
+
+    for phrase, scores in phrase_scores.items():
+        linking_score_map[phrase] = float(np.mean(scores))
+    if link_top_k:
+        linking_score_map = dict(sorted(linking_score_map.items(), key=lambda x: x[1], reverse=True)[:link_top_k])
+        top_k_phrases_keys = {compute_mdhash_id(content=p, prefix="entity-") for p in linking_score_map}
+        phrase_weights = {v: w for v, w in phrase_weights.items() if phrase_keys[v] in top_k_phrases_keys}
+        assert sum(1 for w in phrase_weights.values() if w != 0) == len(linking_score_map.keys())
+
+    dpr_sorted_doc_ids, dpr_sorted_doc_scores = self.dense_passage_retrieval(query)
+    normalized_dpr_sorted_scores = retrieval.min_max_normalize(dpr_sorted_doc_scores)
+    phrase_dense = np.zeros(n_vertices)
+    if phrase_weights:
+        phrase_dense[np.fromiter(phrase_weights.keys(), dtype=np.int64)] = np.fromiter(phrase_weights.values(),
+                                                                                   dtype=np.float64)
+    passage_weights = np.zeros(n_vertices)
+    passage_weights[_passage_vertices(self)[np.asarray(dpr_sorted_doc_ids, dtype=np.int64)]] = \
+        normalized_dpr_sorted_scores * passage_node_weight
+    node_weights = phrase_dense + passage_weights
+
+    assert np.sum(node_weights) > 0, f'No phrases found in the graph for the given facts: {top_k_facts}'
+    ppr_sorted_doc_ids, ppr_sorted_doc_scores = self.run_ppr(node_weights)
+    assert len(ppr_sorted_doc_ids) == len(
+        self.passage_node_idxs), f"Doc prob length {len(ppr_sorted_doc_ids)} != corpus length {len(self.passage_node_idxs)}"
+    return ppr_sorted_doc_ids, ppr_sorted_doc_scores, used_phrases_with_scores
+
+
+GRAPH_METHODS = {
+    "graph_search_with_fact_entities": graph_search_with_fact_entities,
+    "run_ppr": run_ppr,
 }

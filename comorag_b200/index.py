@@ -388,25 +388,9 @@ class DenseIndex:
 
     def rank_device(self, scores_row: torch.Tensor, stream: Optional[torch.cuda.Stream] = None
                     ) -> Tuple[torch.Tensor, torch.Tensor]:
-        """Full descending ranking of one fp32 score row on the device (crag_rank_scores; ties by ascending row):
-        np.argsort(scores)[::-1] + the gather of ComoRAG.py:965-966.  Returns (ids int64 [n], scores fp32 [n])."""
-        if scores_row.dtype != torch.float32 or scores_row.dim() != 1 or not scores_row.is_contiguous():
-            raise ValueError("scores_row must be a contiguous fp32 vector")
-        n = scores_row.shape[0]
-        lib = _native.load()
-        dev = self.device
-        with torch.cuda.device(dev):
-            st = stream if stream is not None else torch.cuda.current_stream(dev)
-            with torch.cuda.stream(st):
-                ids = torch.empty((n,), dtype=torch.int64, device=dev)
-                out = torch.empty((n,), dtype=torch.float32, device=dev)
-                if n:
-                    ws_bytes = lib.crag_rank_workspace_bytes(n)
-                    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-                    rc = lib.crag_rank_scores(scores_row.data_ptr(), n, ids.data_ptr(), out.data_ptr(), ws.data_ptr(),
-                                              ws_bytes, st.cuda_stream)
-                    _native.check(rc, "crag_rank_scores")
-        return ids, out
+        """rank_scores() of one fp32 score row of this index (np.argsort(scores)[::-1] + the gather of
+        ComoRAG.py:965-966)."""
+        return rank_scores(scores_row, stream)
 
     def session(self, nq: int, k: int, use_graph: bool = True) -> "SearchSession":
         """A reusable, CUDA-graph-captured search step for (nq, k); see SearchSession."""
@@ -527,6 +511,29 @@ class SearchSession:
             else:
                 self._enqueue(torch.cuda.current_stream(dev))
         return self.ids, self.scores, self.minmax
+
+
+def rank_scores(scores_row: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Full descending ranking of one device fp32 score vector (crag_rank_scores; ties by ascending row):
+    np.argsort(scores)[::-1] + the gather of ComoRAG.py:965-966 for passage scores, and of ComoRAG.py:1101-1102 for
+    PPR scores.  Returns (ids int64 [n], scores fp32 [n]) on the vector's device."""
+    if scores_row.dtype != torch.float32 or scores_row.dim() != 1 or not scores_row.is_contiguous():
+        raise ValueError("scores_row must be a contiguous fp32 vector")
+    n = scores_row.shape[0]
+    lib = _native.load()
+    dev = scores_row.device
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        with torch.cuda.stream(st):
+            ids = torch.empty((n,), dtype=torch.int64, device=dev)
+            out = torch.empty((n,), dtype=torch.float32, device=dev)
+            if n:
+                ws_bytes = lib.crag_rank_workspace_bytes(n)
+                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+                rc = lib.crag_rank_scores(scores_row.data_ptr(), n, ids.data_ptr(), out.data_ptr(), ws.data_ptr(),
+                                          ws_bytes, st.cuda_stream)
+                _native.check(rc, "crag_rank_scores")
+    return ids, out
 
 
 def merge_topk(scores: torch.Tensor, ids: torch.Tensor, minmax: Optional[torch.Tensor]):

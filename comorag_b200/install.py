@@ -20,12 +20,14 @@ from typing import Dict
 
 
 def install(package: str = "src.comorag", rerank: bool = False, summaries: bool = True, search: bool = True,
-            knn: bool = True, encoder: bool = True) -> Dict[str, int]:
+            knn: bool = True, encoder: bool = True, graph: bool = False) -> Dict[str, int]:
     """Returns {name: number of module attributes (or class methods) rebound}.  `rerank=True` also swaps the LLM
     filter for the dense reranker (new arithmetic, off by default so answers stay reference-identical); `search`
     rebinds the four ComoRAG retrieval methods, `knn` the synonymy-edge retrieve_knn; `encoder=False` keeps the
     reference's own embedding model class (HF, fp32) and swaps only the store / search half -- the parity tests use
-    that to compare rankings without the bf16 encoder's error in the way."""
+    that to compare rankings without the bf16 encoder's error in the way.  `graph=True` also rebinds
+    graph_search_with_fact_entities and run_ppr (comorag_methods.GRAPH_METHODS: PPR on the device, crag_ppr); it
+    needs a real igraph.Graph (get_edgelist, es["weight"]) and is off by default."""
     from . import embedding_model as em
     from . import embedding_store as es
     from . import rerank as rr
@@ -54,15 +56,18 @@ def install(package: str = "src.comorag", rerank: bool = False, summaries: bool 
             if getattr(mod, attr, None) is old:
                 setattr(mod, attr, new)
                 counts[attr] += 1
-    if search:
+    if search or graph:
         from . import comorag_methods as cm
         main = sys.modules.get(package + ".ComoRAG") or importlib.import_module(package + ".ComoRAG")
         cls = main.ComoRAG
+        methods = {**(cm.METHODS if search else {}), **(cm.GRAPH_METHODS if graph else {})}
         originals = cls.__dict__.get("_comorag_b200_originals")
         if originals is None:
-            originals = {name: cls.__dict__[name] for name in cm.METHODS}
+            originals = {}
             cls._comorag_b200_originals = originals       # uninstall() / the parity tests can reach the reference methods
-        for name, fn in cm.METHODS.items():
+        for name, fn in methods.items():
+            if name not in originals:
+                originals[name] = cls.__dict__[name]
             setattr(cls, name, fn)
             counts["ComoRAG." + name] = 1
     return counts

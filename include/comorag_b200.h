@@ -191,6 +191,26 @@ CRAG_API size_t crag_rank_workspace_bytes(int64_t n);
 CRAG_API int crag_rank_scores(const float* scores, int64_t n, int64_t* out_ids, float* out_scores, void* workspace,
                               size_t workspace_bytes, crag_stream_t stream);
 
+/* Personalized PageRank, the solve of the reference's run_ppr (ComoRAG.py:1086-1105):
+ *     graph.personalized_pagerank(directed=False, weights='weight', damping=d, reset=reset_prob)
+ * on an undirected graph given in CSR "pull" form: row i lists every neighbour j once, ascending, with
+ * coef = W_ij / s_j (W_ij = summed weight of the edges joining i and j, s_j = sum_i W_ij; no self-loops), and a
+ * dangling vertex (s_j = 0, empty row) restarts by the reset.  The result is y_T / sum(y_T) of
+ *     y_0 = (1 - d) v,   y_{t+1} = (1 - d) v + d A y_t          (t < T = iterations)
+ * which is within 2 d^(T+1) / (1 - d) in L1 of the exact PPR (DESIGN.md section 2a).  fp32 arithmetic, merge-path
+ * load balance over rows + nonzeros, no floating-point atomics: the same inputs give bit-identical output on every
+ * run and stream.
+ *   row_ptr device int64 [n_vertices + 1]; col device int32 [nnz]; coef device fp32 [nnz]; 1 <= n_vertices < 2^31
+ *   reset device fp32 [n_vertices], >= 0, sum 1; damping in [0, 1); iterations T >= 0
+ *   out_vertices device int32 [n_out], each in [0, n_vertices), or NULL with n_out = n_vertices (all vertices)
+ *   out device fp32 [n_out]: out[p] = x[out_vertices[p]]
+ *   workspace >= crag_ppr_workspace_bytes(n_vertices, nnz) bytes, 256-B aligned.
+ * Enqueues 2T + 4 kernels. */
+CRAG_API size_t crag_ppr_workspace_bytes(int64_t n_vertices, int64_t nnz);
+CRAG_API int crag_ppr(const int64_t* row_ptr, const int32_t* col, const float* coef, int64_t n_vertices, int64_t nnz,
+                      const float* reset, float damping, int iterations, const int32_t* out_vertices, int64_t n_out,
+                      float* out, void* workspace, size_t workspace_bytes, crag_stream_t stream);
+
 /* ------------------------------------------------------------------ encoder
  * Dense projection of the encoder forward (BGEEmbedding.py:120 runs it through
  * HF's BertModel: attention.self.{query,key,value}, attention.output.dense,
