@@ -313,15 +313,23 @@ _graph_lock = __import__("threading").Lock()
 
 def _device_graph(self) -> DeviceGraph:
     """self.graph as a DeviceGraph, built on first use and cached on the instance, keyed by (vcount, ecount): the
-    reference only ever adds vertices and edges (ComoRAG.py:779-841), so a changed graph changes one of the two."""
+    reference only ever adds vertices and edges (ComoRAG.py:779-841), so a changed graph changes one of the two.
+    The graph it builds coalesces the PPR of concurrent graph searches (DeviceGraph.enable_batching: one
+    crag_ppr_batch pass for the questions ComoRAG.py:436-441 answers together, each result bit-identical to its own
+    crag_ppr call); a rebuild closes the old graph's batcher, and calls still on their way to it run directly."""
     key = (self.graph.vcount(), self.graph.ecount())
     cached = getattr(self, "_crag_graph", None)
     if cached is None or cached[0] != key:
         with _graph_lock:               # up to 16 tri_retrieve threads reach the first graph search together
             cached = getattr(self, "_crag_graph", None)
             if cached is None or cached[0] != key:
-                cached = (key, DeviceGraph.from_igraph(self.graph))
+                old = cached
+                graph = DeviceGraph.from_igraph(self.graph)
+                graph.enable_batching()
+                cached = (key, graph)
                 self._crag_graph = cached
+                if old is not None:
+                    old[1].disable_batching()
     return cached[1]
 
 

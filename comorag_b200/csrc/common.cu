@@ -86,7 +86,7 @@ int sm_count() {
 
 }  // namespace crag
 
-extern "C" int crag_version(void) { return 1002; }
+extern "C" int crag_version(void) { return 1003; }
 extern "C" const char* crag_last_error(void) { return crag::g_err; }
 extern "C" int crag_sm_count(void) { return crag::sm_count(); }
 

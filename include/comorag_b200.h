@@ -211,6 +211,20 @@ CRAG_API int crag_ppr(const int64_t* row_ptr, const int32_t* col, const float* c
                       const float* reset, float damping, int iterations, const int32_t* out_vertices, int64_t n_out,
                       float* out, void* workspace, size_t workspace_bytes, crag_stream_t stream);
 
+/* Multi-source Personalized PageRank: crag_ppr for `batch` resets over the same graph in one pass per iteration
+ * (a CSR x dense-block product, y stored vertex-major [n_vertices][W] with W the batch rounded up to 2, 4, 8, 16
+ * or 32).  Column b of the output is bit-identical to crag_ppr(..., resets + b * n_vertices, ...) with the same
+ * graph, damping, iterations and out_vertices.
+ *   resets device fp32 [batch][n_vertices], each row >= 0, sum 1; 1 <= batch <= 32
+ *   out    device fp32 [batch][n_out], query-major: out[b * n_out + p] = x_b[out_vertices[p]]
+ *   workspace >= crag_ppr_batch_workspace_bytes(n_vertices, nnz, batch) bytes, 256-B aligned.
+ * Every other argument, rule and error as crag_ppr.  Enqueues 2T + 5 kernels. */
+CRAG_API size_t crag_ppr_batch_workspace_bytes(int64_t n_vertices, int64_t nnz, int batch);
+CRAG_API int crag_ppr_batch(const int64_t* row_ptr, const int32_t* col, const float* coef, int64_t n_vertices,
+                            int64_t nnz, const float* resets, int batch, float damping, int iterations,
+                            const int32_t* out_vertices, int64_t n_out, float* out, void* workspace,
+                            size_t workspace_bytes, crag_stream_t stream);
+
 /* ------------------------------------------------------------------ encoder
  * Dense projection of the encoder forward (BGEEmbedding.py:120 runs it through
  * HF's BertModel: attention.self.{query,key,value}, attention.output.dense,
