@@ -44,8 +44,9 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
-int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride_bytes,
-                      uint32_t box_rows, uint32_t box_cols) {
+namespace {
+int make_tmap_2d(CUtensorMap* out, CUtensorMapDataType type, const void* base, uint64_t rows, uint64_t cols,
+                 uint64_t row_stride_bytes, uint32_t box_rows, uint32_t box_cols) {
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return fail(CRAG_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (driver too old?)");
   if (rows == 0 || cols == 0) return fail(CRAG_ERR_INVALID, "tensor map over an empty tensor");
@@ -53,7 +54,7 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
   const cuuint64_t gstride[1] = {row_stride_bytes};
   const cuuint32_t box[2] = {box_cols, box_rows};
   const cuuint32_t estride[2] = {1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estride,
+  CUresult r = enc(out, type, 2, const_cast<void*>(base), gdim, gstride, box, estride,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
@@ -61,6 +62,17 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
                 int(r), (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)row_stride_bytes,
                 box_rows, box_cols);
   return CRAG_OK;
+}
+}  // namespace
+
+int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride_bytes,
+                      uint32_t box_rows, uint32_t box_cols) {
+  return make_tmap_2d(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rows, cols, row_stride_bytes, box_rows, box_cols);
+}
+
+int make_tmap_u8_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride_bytes,
+                    uint32_t box_rows, uint32_t box_cols) {
+  return make_tmap_2d(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rows, cols, row_stride_bytes, box_rows, box_cols);
 }
 
 int sm_count() {

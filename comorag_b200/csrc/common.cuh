@@ -29,6 +29,9 @@ int fail(int code, const char* fmt, ...);
 // out-of-bounds elements read as zero.
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                       uint64_t row_stride_bytes, uint32_t box_rows, uint32_t box_cols = 64);
+// The same for int8 / uint8 elements: box = box_rows x 128 columns, again one 128-byte swizzle span.
+int make_tmap_u8_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride_bytes,
+                    uint32_t box_rows, uint32_t box_cols = 128);
 
 int sm_count();
 

@@ -1,0 +1,56 @@
+// Int8 corpus shards: C entries of the quantiser and of the exact bf16 rescore (quant_kernels.cuh).  The int8 scan
+// between them, crag_search_topk_i8, is the I8 variant of the shard scan in search.cu.
+#include "common.cuh"
+#include "quant_kernels.cuh"
+
+using namespace crag;
+
+extern "C" int crag_quantize_rows_i8(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, void* out_i8,
+                                     int64_t out_stride, float* out_scales, crag_stream_t stream) {
+  if (dim < 1 || dim > 1024) return fail(CRAG_ERR_INVALID, "quantize_i8: dim must be in [1, 1024] (dim=%d)", dim);
+  const int dim8 = (dim + 127) / 128 * 128;
+  if (n_rows < 0 || n_rows >= (int64_t(1) << 31)) return fail(CRAG_ERR_INVALID, "quantize_i8: n_rows out of range (%lld)", (long long)n_rows);
+  if (row_stride < dim) return fail(CRAG_ERR_INVALID, "quantize_i8: row_stride must be >= dim");
+  if (out_stride < dim8 || out_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "quantize_i8: out_stride must be >= %d and a multiple of 16", dim8);
+  if (n_rows == 0) return CRAG_OK;
+  if (!rows_bf16 || !out_i8 || !out_scales) return fail(CRAG_ERR_INVALID, "quantize_i8: null pointer");
+  if ((reinterpret_cast<uintptr_t>(rows_bf16) & 1) || (reinterpret_cast<uintptr_t>(out_i8) & 15)) return fail(CRAG_ERR_INVALID, "quantize_i8: rows must be 2-byte and out 16-byte aligned");
+  const int64_t grid = (n_rows + kQuantThreads / 32 - 1) / (kQuantThreads / 32);
+  quantize_rows_kernel<<<unsigned(grid), kQuantThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint16_t*>(rows_bf16), n_rows, dim, row_stride, dim8, static_cast<int8_t*>(out_i8), out_stride, out_scales);
+  CRAG_CUDA_OK(cudaGetLastError());
+  return CRAG_OK;
+}
+
+extern "C" int crag_rescore_topk(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, int64_t row_offset,
+                                 const void* queries_bf16, int nq, const int64_t* cand_ids, int n_cand, int k,
+                                 int64_t* out_ids, float* out_scores, crag_stream_t stream) {
+  if (nq < 1 || n_cand < 1 || n_cand > kRescoreMaxCand || k < 1 || k > n_cand) return fail(CRAG_ERR_INVALID, "rescore: need nq >= 1 and 1 <= k <= n_cand <= %d (nq=%d n_cand=%d k=%d)", kRescoreMaxCand, nq, n_cand, k);
+  if (dim < 8 || dim > 1024 || dim % 8 != 0) return fail(CRAG_ERR_INVALID, "rescore: dim must be a multiple of 8 in [8, 1024] (dim=%d)", dim);
+  if (n_rows < 0 || n_rows >= (int64_t(1) << 31) || row_offset < 0) return fail(CRAG_ERR_INVALID, "rescore: need 0 <= n_rows < 2^31 and row_offset >= 0");
+  if (row_stride < dim || row_stride % 8 != 0) return fail(CRAG_ERR_INVALID, "rescore: row_stride must be >= dim and a multiple of 8");
+  if (!queries_bf16 || !cand_ids || !out_ids || !out_scores || (n_rows > 0 && !rows_bf16)) return fail(CRAG_ERR_INVALID, "rescore: null pointer");
+  if ((reinterpret_cast<uintptr_t>(rows_bf16) | reinterpret_cast<uintptr_t>(queries_bf16)) & 15) return fail(CRAG_ERR_INVALID, "rescore: rows/queries must be 16-byte aligned");
+  // The rows may be device memory or page-locked host memory reached through unified addressing.  A kernel that
+  // dereferences pageable host memory faults, so anything else is refused here, before a launch.
+  const void* rows = rows_bf16;
+  if (n_rows > 0) {
+    cudaPointerAttributes attr;
+    const cudaError_t e = cudaPointerGetAttributes(&attr, rows_bf16);
+    if (e != cudaSuccess) {
+      cudaGetLastError();   // the failed query must not surface at the caller's next cudaGetLastError
+      return fail(CRAG_ERR_INVALID, "rescore: rows are not memory the device can read (%s)", cudaGetErrorString(e));
+    }
+    if (attr.type == cudaMemoryTypeHost) {
+      if (!attr.devicePointer) return fail(CRAG_ERR_INVALID, "rescore: page-locked rows are not mapped into the device's address space");
+      rows = attr.devicePointer;
+    } else if (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged) {
+      return fail(CRAG_ERR_INVALID, "rescore: rows must be device memory or page-locked host memory (pageable host memory given)");
+    }
+  }
+  rescore_topk_kernel<<<nq, kRescoreThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint16_t*>(rows), n_rows, dim, row_stride, row_offset, static_cast<const uint16_t*>(queries_bf16),
+      cand_ids, n_cand, k, out_ids, out_scores);
+  CRAG_CUDA_OK(cudaGetLastError());
+  return CRAG_OK;
+}

@@ -1,0 +1,121 @@
+// Int8 corpus shards: the row / query quantiser and the exact bf16 rescore of the int8 scan's candidates (quant.cu).
+// Pure SIMT, so tests/warp_emu can run both kernels on the CPU.  Semantics (oracle/quant_oracle.py, DESIGN.md 3e):
+//
+//   quantise  a bf16 row x of width dim becomes int8 [dim8 = ceil(dim / 128) * 128], zero padded, and one fp32 scale
+//             s = amax / 127 (amax = max |x_i|, division rounded to nearest);  x^_i = clamp(rint(x_i / s), -127, 127)
+//             with rint rounding half to even; s = 0 gives a zero row.  Queries are quantised the same way.
+//   rescore   each candidate's score is recomputed as the fp32 dot of its bf16 row and the bf16 query in one pinned
+//             order: lane l of a warp takes the 16-byte chunks l, l + 32, ...; inside a chunk each product (rounded)
+//             is added to the lane's partial (rounded) in element order from 0.f; the partials are combined by an
+//             xor-shuffle tree over 16, 8, 4, 2, 1.  The result is the top k of the candidates by (score descending,
+//             row ascending), as make_key orders them.
+#pragma once
+#include <math.h>
+#include <stdint.h>
+#include <cuda_runtime.h>
+
+#include "topk.cuh"
+
+namespace crag {
+
+constexpr int kQuantThreads = 256;           // quantiser: one warp per row
+constexpr int kQuantClamp = 127;             // int8 codes are symmetric: -127 .. 127
+constexpr int kRescoreThreads = 256;         // rescore: one CTA per query, one warp per candidate
+constexpr int kRescoreMaxCand = 128;         // candidates per query: one warp sorts them, 4 keys per lane
+
+__device__ __forceinline__ float bf16_bits_to_f32(uint32_t bits16) { return __uint_as_float(bits16 << 16); }
+
+// x^ of one element under scale s (s != 0)
+__device__ __forceinline__ int quant_value(float x, float s) {
+  int v = __float2int_rn(__fdiv_rn(x, s));
+  v = v < -kQuantClamp ? -kQuantClamp : v;
+  return v > kQuantClamp ? kQuantClamp : v;
+}
+
+// rows: bf16 bits [n_rows, row_stride], dim valid columns.  out: int8 [n_rows, out_stride], dim8 columns written
+// (dim8 a multiple of 128, out 4-byte aligned, out_stride a multiple of 4), scales: fp32 [n_rows].
+__global__ void __launch_bounds__(kQuantThreads)
+quantize_rows_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride, int dim8,
+                     int8_t* __restrict__ out, int64_t out_stride, float* __restrict__ scales) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = int64_t(blockIdx.x) * (kQuantThreads / 32) + (threadIdx.x >> 5);
+  if (row >= n_rows) return;   // warp-uniform
+  const uint16_t* x = rows + row * row_stride;
+  // |x| as bits: for non-negative finite floats the unsigned order of the bits is the order of the values
+  uint32_t amax_bits = 0;
+  for (int c = lane; c < dim; c += 32) {
+    const uint32_t a = uint32_t(x[c] & 0x7FFFu) << 16;
+    amax_bits = a > amax_bits ? a : amax_bits;
+  }
+  amax_bits = __reduce_max_sync(0xffffffffu, amax_bits);
+  const float s = __fdiv_rn(__uint_as_float(amax_bits), 127.f);
+  int8_t* o = out + row * out_stride;
+  for (int c0 = lane * 4; c0 < dim8; c0 += 128) {
+    uint32_t packed = 0;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int c = c0 + e;
+      const int v = (c < dim && s != 0.f) ? quant_value(bf16_bits_to_f32(x[c]), s) : 0;
+      packed |= uint32_t(uint8_t(int8_t(v))) << (8 * e);
+    }
+    *reinterpret_cast<uint32_t*>(o + c0) = packed;
+  }
+  if (lane == 0) scales[row] = s;
+}
+
+// partial += a_i * b_i over the 8 bf16 of one 16-byte chunk, in element order (the low half of a word comes first)
+__device__ __forceinline__ float dot_chunk(float partial, const uint4& a, const uint4& b) {
+  const uint32_t wa[4] = {a.x, a.y, a.z, a.w}, wb[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+  for (int w = 0; w < 4; ++w) {
+    partial = __fadd_rn(partial, __fmul_rn(__uint_as_float(wa[w] << 16), __uint_as_float(wb[w] << 16)));
+    partial = __fadd_rn(partial, __fmul_rn(__uint_as_float(wa[w] & 0xFFFF0000u), __uint_as_float(wb[w] & 0xFFFF0000u)));
+  }
+  return partial;
+}
+
+// One CTA per query.  rows: bf16 [n_rows, row_stride] (device or page-locked host memory), queries: bf16 [nq, dim]
+// dense, dim a multiple of 8, rows and queries 16-byte aligned.  cand_ids: int64 [nq, n_cand] global ids; an id outside
+// [row_offset, row_offset + n_rows) -- -1 among them -- is no candidate and its row is never read.  Writes the top k
+// (k <= n_cand <= 128) to out_ids / out_scores [nq, k], -1 / -inf past the valid candidates.
+__global__ void __launch_bounds__(kRescoreThreads)
+rescore_topk_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride, int64_t row_offset,
+                    const uint16_t* __restrict__ queries, const int64_t* __restrict__ cand_ids, int n_cand, int k,
+                    int64_t* __restrict__ out_ids, float* __restrict__ out_scores) {
+  __shared__ uint64_t keys[kRescoreMaxCand];
+  const int q = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint16_t* qv = queries + int64_t(q) * dim;
+  const int n_chunks = dim / 8;
+  for (int c = warp; c < kRescoreMaxCand; c += kRescoreThreads / 32) {
+    uint64_t key = 0;   // no candidate
+    const int64_t local = c < n_cand ? __ldg(&cand_ids[int64_t(q) * n_cand + c]) - row_offset : -1;
+    if (local >= 0 && local < n_rows) {   // warp-uniform
+      const uint16_t* xr = rows + local * row_stride;
+      float partial = 0.f;
+#pragma unroll 4
+      for (int ch = lane; ch < n_chunks; ch += 32)
+        partial = dot_chunk(partial, *reinterpret_cast<const uint4*>(xr + ch * 8), __ldg(reinterpret_cast<const uint4*>(qv + ch * 8)));
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) partial = __fadd_rn(partial, __shfl_xor_sync(0xffffffffu, partial, o));
+      key = make_key(partial, uint32_t(local));
+    }
+    if (lane == 0) keys[c] = key;
+  }
+  __syncthreads();
+  if (warp != 0) return;
+  constexpr int EPL = kRescoreMaxCand / 32;
+  uint64_t v[EPL];
+#pragma unroll
+  for (int j = 0; j < EPL; ++j) v[j] = keys[lane * EPL + j];
+  warp_sort_desc<EPL>(v, lane);
+#pragma unroll
+  for (int j = 0; j < EPL; ++j) {
+    const int g = lane * EPL + j;
+    if (g < k) {
+      out_ids[int64_t(q) * k + g] = v[j] ? int64_t(key_id(v[j])) + row_offset : -1;
+      out_scores[int64_t(q) * k + g] = v[j] ? key_score(v[j]) : -INFINITY;
+    }
+  }
+}
+
+}  // namespace crag

@@ -80,12 +80,26 @@ struct SmemScoreTiles {
   }
 };
 
-template <int KLIST, int CAP, int STAGES, bool IVF = false, bool SCORES = false>
+// Int8 variant of the flat top-k scan (I8 = true, crag_search_topk_i8): the shard and the query block are int8 with one
+// fp32 scale per row / query (quant_kernels.cuh).  A 128-byte swizzle row holds 128 int8 instead of 64 bf16, so boxes,
+// stages, descriptors and score tiles keep their byte sizes; the warpgroup issues m64n32k32.s32.s8.s8 and its epilogue
+// writes S1 = float(acc) * (s_q * s_row) to the score tile, which the select warps rank as they rank bf16 scores.
+struct I8Args {
+  const float* row_scales;     // [n_rows]
+  const float* query_scales;   // [nq] of this pass
+};
+template <bool IVF, bool SCORES, bool I8> struct ScanParam { using type = typename IvfParam<IVF, SCORES>::type; };
+template <> struct ScanParam<false, false, true> { using type = I8Args; };
+
+template <int KLIST, int CAP, int STAGES, bool IVF = false, bool SCORES = false, bool I8 = false>
 __global__ void __launch_bounds__(kSearchThreads, 1)
 search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_constant__ CUtensorMap tm_q,
                    int n_rows, int num_kb, int nq, int k, const uint64_t* __restrict__ after_keys,
                    uint64_t* __restrict__ pool, uint32_t perm_mul, int perm_shift, uint64_t* __restrict__ part_keys,
-                   float* __restrict__ part_minmax, const typename IvfParam<IVF, SCORES>::type args) {
+                   float* __restrict__ part_minmax, const typename ScanParam<IVF, SCORES, I8>::type args) {
+  static_assert(!I8 || (!IVF && !SCORES), "the int8 scan is a flat top-k scan");
+  // elements per 128-byte swizzle row: the producer's column step per k-block
+  constexpr int kBlockElems = I8 ? 128 : kBlockK;
   using L = SearchLayout<KLIST, CAP, STAGES>;
   static_assert(L::smem_bytes() <= 227 * 1024, "stages, score tiles and candidate lists exceed 227 KB of shared memory");
   extern __shared__ uint8_t smem_raw[];
@@ -138,8 +152,8 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
           if constexpr (IVF) tile_row0 = __ldg(&args.work[tile].x);
           else tile_row0 = tile * kTileRows;
           uint8_t* st = stage_base + stage * kStageTotalBytes;
-          tma_load_2d_hint(&tm_corpus, &bar_full[stage], st, kb * kBlockK, tile_row0, pol);
-          tma_load_2d(&tm_q, &bar_full[stage], st + kStageBytes, kb * kBlockK, 0);
+          tma_load_2d_hint(&tm_corpus, &bar_full[stage], st, kb * kBlockElems, tile_row0, pol);
+          tma_load_2d(&tm_q, &bar_full[stage], st + kStageBytes, kb * kBlockElems, 0);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -153,10 +167,32 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
     uint32_t phase = 0;
     int acc = 0;
     uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      float d[2][16];
+    using Acc = std::conditional_t<I8, int32_t, float>;
+    // I8: the scales of this thread's 8 query columns (0 past nq), held for the whole scan
+    float q_scale[I8 ? kNQ / 4 : 1];
+    if constexpr (I8) {
 #pragma unroll
-      for (int i = 0; i < 16; ++i) d[0][i] = d[1][i] = 0.f;
+      for (int j = 0; j < kNQ / 8; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int q = 8 * j + frag_col + c;
+          q_scale[2 * j + c] = q < nq ? __ldg(&args.query_scales[q]) : 0.f;
+        }
+    }
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      Acc d[2][16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) d[0][i] = d[1][i] = Acc(0);
+      // I8: the scales of this thread's 4 rows of the tile (0 past n_rows), fetched while the k-blocks stream in
+      float r_scale[I8 ? 4 : 1];
+      if constexpr (I8) {
+        const int row0 = order(tile) * kTileRows;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int row = row0 + (i >> 1) * 64 + frag_row + (i & 1) * 8;
+          r_scale[i] = row < n_rows ? __ldg(&args.row_scales[row]) : 0.f;
+        }
+      }
       int prev = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&bar_full[stage], phase);
@@ -164,10 +200,15 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
         const uint32_t b_addr = a_addr + kStageBytes;
         wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < kBlockK / 16; ++ks) {
+        for (int ks = 0; ks < kBlockK / 16; ++ks) {   // 32-byte K steps: 16 bf16 or 32 int8
           const uint64_t db = wgmma_desc_sw128(b_addr + ks * 32);
-          wgmma_m64n32k16_ss(d[0], wgmma_desc_sw128(a_addr + ks * 32), db, 1u);
-          wgmma_m64n32k16_ss(d[1], wgmma_desc_sw128(a_addr + 64 * 128 + ks * 32), db, 1u);
+          if constexpr (I8) {
+            wgmma_m64n32k32_s8_ss(d[0], wgmma_desc_sw128(a_addr + ks * 32), db, 1u);
+            wgmma_m64n32k32_s8_ss(d[1], wgmma_desc_sw128(a_addr + 64 * 128 + ks * 32), db, 1u);
+          } else {
+            wgmma_m64n32k16_ss(d[0], wgmma_desc_sw128(a_addr + ks * 32), db, 1u);
+            wgmma_m64n32k16_ss(d[1], wgmma_desc_sw128(a_addr + 64 * 128 + ks * 32), db, 1u);
+          }
         }
         wgmma_commit();
         wgmma_wait<1>();   // k-block kb - 1 has retired: its smem slot goes back to the producer
@@ -188,7 +229,12 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             const int row = m * 64 + frag_row + (i >> 1) * 8;
-            st[score_slot(row, 8 * j + frag_col + (i & 1))] = d[m][4 * j + i];
+            if constexpr (I8) {   // S1 = float(acc) * (s_q * s_row); |acc| <= 127^2 * 1024 < 2^24 converts exactly
+              const float scale = __fmul_rn(q_scale[2 * j + (i & 1)], r_scale[2 * m + (i >> 1)]);
+              st[score_slot(row, 8 * j + frag_col + (i & 1))] = __fmul_rn(__int2float_rn(d[m][4 * j + i]), scale);
+            } else {
+              st[score_slot(row, 8 * j + frag_col + (i & 1))] = d[m][4 * j + i];
+            }
           }
       mbar_arrive(&bar_tfull[acc]);
       if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
@@ -196,7 +242,8 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
   } else {
     // ================================================================== select
     SmemScoreTiles tiles{score_tiles, bar_tfull, bar_tempty};
-    select_warps<KLIST, CAP, IVF, SCORES>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, args, warp, lane);
+    if constexpr (I8) select_warps<KLIST, CAP, false, false>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, NoIvfArgs{}, warp, lane);
+    else select_warps<KLIST, CAP, IVF, SCORES>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, args, warp, lane);
   }
 }
 
@@ -221,12 +268,12 @@ SearchPlan plan_search(int k) {
 }
 
 // One launch of the scan.  The dynamic shared-memory limit is raised once per instantiation and device.
-template <int KLIST, int CAP, int STAGES, bool IVF, bool SCORES>
+template <int KLIST, int CAP, int STAGES, bool IVF, bool SCORES, bool I8 = false>
 int launch_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k, int grid,
                 const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift, uint64_t* part_keys,
-                float* part_minmax, const typename IvfParam<IVF, SCORES>::type& args, cudaStream_t stream) {
+                float* part_minmax, const typename ScanParam<IVF, SCORES, I8>::type& args, cudaStream_t stream) {
   constexpr size_t smem = SearchLayout<KLIST, CAP, STAGES>::smem_bytes();
-  auto kern = search_topk_kernel<KLIST, CAP, STAGES, IVF, SCORES>;
+  auto kern = search_topk_kernel<KLIST, CAP, STAGES, IVF, SCORES, I8>;
   static bool attr_set[64] = {};
   int dev = 0;
   CRAG_CUDA_OK(cudaGetDevice(&dev));
@@ -240,12 +287,14 @@ int launch_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_row
 }
 
 // A top-k scan with the selector of k: 64-key lists and 6 stages up to k = 64, 128-key lists and 4 stages above.
+// I8Args selects the int8 scan.
 template <bool IVF, class Args>
 int launch_topk_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k,
                      int grid, const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift,
                      uint64_t* part_keys, float* part_minmax, const Args& args, cudaStream_t stream) {
-  if (k <= 64) return launch_scan<64, 64, 6, IVF, false>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
-  return launch_scan<128, 128, 4, IVF, false>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+  constexpr bool I8 = std::is_same<Args, I8Args>::value;
+  if (k <= 64) return launch_scan<64, 64, 6, IVF, false, I8>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+  return launch_scan<128, 128, 4, IVF, false, I8>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
 }
 
 // The merge kernels' list size for k (32, 64 or 128), passed to `launch` as a std::integral_constant.
@@ -298,10 +347,11 @@ inline int scan_grid(int64_t n_rows, const SearchPlan& plan) {
 // the flat scans permute groups of 2^kPermShift consecutive tiles (TileOrder)
 constexpr int kPermShift = 3;
 
-// one corpus pass for queries q0 .. q0 + nq - 1 (nq <= 32): per-CTA partial lists into the workspace
+// one corpus pass for queries q0 .. q0 + nq - 1 (nq <= 32): per-CTA partial lists into the workspace.  With `i8` the
+// corpus and queries are int8 [*, dim] (dim a multiple of 128) with the scales of i8 (query scales from query 0 on).
 int scan_pass(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride, const void* queries, int q0,
               int nq, int k, const uint64_t* after_keys, void* workspace, size_t workspace_bytes,
-              const SearchPlan& plan, cudaStream_t stream) {
+              const SearchPlan& plan, cudaStream_t stream, const I8Args* i8 = nullptr) {
   const int grid = scan_grid(n_rows, plan);
   if (grid == 0) return CRAG_OK;
   uint64_t* part_keys = static_cast<uint64_t*>(workspace);
@@ -314,6 +364,15 @@ int scan_pass(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_st
     CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, plan.pool_bytes, stream));
   }
   CUtensorMap tm_corpus, tm_q;
+  if (i8) {
+    int rc = make_tmap_u8_2d(&tm_corpus, corpus, uint64_t(n_rows), uint64_t(dim), uint64_t(corpus_row_stride), kTileRows);
+    if (rc != CRAG_OK) return rc;
+    rc = make_tmap_u8_2d(&tm_q, static_cast<const uint8_t*>(queries) + size_t(q0) * dim, uint64_t(nq), uint64_t(dim), uint64_t(dim), kNQ);
+    if (rc != CRAG_OK) return rc;
+    return launch_topk_scan<false>(tm_corpus, tm_q, int(n_rows), dim / 128, nq, k, grid, after_keys, pool,
+                                   perm_multiplier(num_tiles >> kPermShift), kPermShift, part_keys, part_minmax,
+                                   I8Args{i8->row_scales, i8->query_scales + q0}, stream);
+  }
   int rc = make_tmap_bf16_2d(&tm_corpus, corpus, uint64_t(n_rows), uint64_t(dim), uint64_t(corpus_row_stride) * 2, kTileRows);
   if (rc != CRAG_OK) return rc;
   rc = make_query_tmap(&tm_q, queries, q0, nq, dim);
@@ -467,6 +526,33 @@ extern "C" int crag_search_topk(const void* corpus, int64_t n_rows, int dim, int
                                 crag_stream_t stream) {
   return crag_search_topk_after(corpus, n_rows, dim, corpus_row_stride, row_offset, queries, nq, k, nullptr, out_ids,
                                 out_scores, out_minmax, nullptr, workspace, workspace_bytes, stream);
+}
+
+// ------------------------------------------------------------------ int8 shards (quant_kernels.cuh)
+extern "C" int crag_search_topk_i8(const void* corpus_i8, const float* row_scales, int64_t n_rows, int dim8,
+                                   int64_t row_stride, int64_t row_offset, const void* queries_i8,
+                                   const float* query_scales, int nq, int k, int64_t* out_ids, float* out_scores,
+                                   float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1);
+  if (nq < 1 || k < 1 || k > 128) return fail(CRAG_ERR_INVALID, "search_i8: need nq >= 1 and 1 <= k <= 128 (nq=%d k=%d)", nq, k);
+  if (dim8 < 128 || dim8 > 1024 || dim8 % 128 != 0) return fail(CRAG_ERR_INVALID, "search_i8: dim8 must be a multiple of 128 in [128, 1024] (dim8=%d)", dim8);
+  if (n_rows < 0 || n_rows >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "search_i8: n_rows out of range (%lld)", (long long)n_rows);
+  if (row_stride < dim8 || row_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "search_i8: row_stride must be >= dim8 and a multiple of 16");
+  if (!queries_i8 || !query_scales || !workspace || !out_ids || !out_scores || (n_rows > 0 && (!corpus_i8 || !row_scales))) return fail(CRAG_ERR_INVALID, "search_i8: null pointer");
+  if ((reinterpret_cast<uintptr_t>(corpus_i8) | reinterpret_cast<uintptr_t>(queries_i8)) & 15) return fail(CRAG_ERR_INVALID, "search_i8: corpus/queries must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "search_i8: workspace must be 256-byte aligned");
+  if (workspace_bytes < plan.keys_bytes + plan.minmax_bytes) return fail(CRAG_ERR_WORKSPACE, "search_i8: workspace %zu < %zu bytes", workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
+  const I8Args i8{row_scales, query_scales};
+  for (int q0 = 0; q0 < nq; q0 += kNQ) {
+    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
+    int rc = scan_pass(corpus_i8, n_rows, dim8, row_stride, queries_i8, q0, nqc, k, nullptr, workspace, workspace_bytes, plan, stream, &i8);
+    if (rc != CRAG_OK) return rc;
+    rc = finalize_pass(workspace, n_rows, nqc, k, row_offset, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
+                       out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, nullptr, plan, stream);
+    if (rc != CRAG_OK) return rc;
+  }
+  return CRAG_OK;
 }
 
 // ------------------------------------------------------------------ exact top-k for large k / many queries

@@ -1,0 +1,140 @@
+"""Int8 snapshot of a DenseIndex: a scan that reads half the bytes of the bf16 shard, then an exact bf16 rescore.
+
+A search runs crag_search_topk_i8 over the int8 rows for `candidates` rows per query, then crag_rescore_topk
+recomputes each candidate's score from its bf16 row and the bf16 query and keeps the best k.  The returned scores are
+those exact fp32 dots; only the choice of candidates comes from the int8 scores.  The bf16 rows are read for the
+candidates only, so they may live in page-locked host memory (rows="host"), which halves the device footprint again.
+Semantics: DESIGN.md section 3e and oracle/quant_oracle.py.
+"""
+from __future__ import annotations
+
+from typing import Optional, Tuple
+
+import numpy as np
+import torch
+
+from . import _native
+from .index import MAX_K, DenseIndex
+
+
+def _dim8(dim: int) -> int:
+    return (dim + 127) // 128 * 128
+
+
+def quantize_rows(rows: torch.Tensor, dim8: int, stream: Optional[torch.cuda.Stream] = None
+                  ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """crag_quantize_rows_i8 of a device bf16 [n, dim] tensor (unit inner stride): (int8 [n, dim8], fp32 scales [n])."""
+    if rows.dtype != torch.bfloat16 or rows.dim() != 2 or not rows.is_cuda or (rows.shape[0] > 1 and rows.stride(1) != 1):
+        raise ValueError("quantize_rows expects a CUDA bf16 [n, dim] tensor with unit inner stride")
+    n, dim = rows.shape
+    dev = rows.device
+    lib = _native.load()
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        with torch.cuda.stream(st):
+            out = torch.empty((n, dim8), dtype=torch.int8, device=dev)
+            scales = torch.empty((n,), dtype=torch.float32, device=dev)
+            rc = lib.crag_quantize_rows_i8(rows.data_ptr() if n else 0, n, dim, rows.stride(0) if n else dim,
+                                           out.data_ptr() if n else 0, dim8, scales.data_ptr() if n else 0,
+                                           st.cuda_stream)
+            _native.check(rc, "crag_quantize_rows_i8")
+    return out, scales
+
+
+class QuantizedIndex:
+    """Frozen int8 snapshot of a DenseIndex's rows (rows added to the DenseIndex later are not seen)."""
+
+    def __init__(self, rows_bf16: torch.Tensor, rows_i8: torch.Tensor, scales: torch.Tensor, dim: int,
+                 device: torch.device, row_offset: int):
+        self._rows = rows_bf16          # [n, dim_pad] bf16, on the device or in page-locked host memory
+        self._i8 = rows_i8              # [n, dim8] int8, device
+        self._scales = scales           # [n] fp32, device
+        self.dim = dim
+        self.dim_pad = rows_bf16.shape[1]
+        self.dim8 = rows_i8.shape[1]
+        self.device = device
+        self.row_offset = row_offset
+
+    @classmethod
+    def from_dense(cls, index: DenseIndex, rows: str = "device") -> "QuantizedIndex":
+        """Quantise the rows `index` holds now.  rows="device" keeps a reference to the index's bf16 buffer;
+        rows="host" copies the bf16 rows into page-locked host memory, so the DenseIndex may be dropped."""
+        if rows not in ("device", "host"):
+            raise ValueError('rows must be "device" or "host"')
+        buf, n = index._snapshot()
+        dev = index.device
+        bf16 = buf[:n]
+        i8, scales = quantize_rows(bf16 if n else torch.zeros((0, index.dim_pad), dtype=torch.bfloat16, device=dev),
+                                   _dim8(index.dim_pad))
+        if rows == "host":
+            host = torch.empty((n, index.dim_pad), dtype=torch.bfloat16, pin_memory=True)
+            if n:
+                host.copy_(bf16)
+            bf16 = host
+        with torch.cuda.device(dev):
+            torch.cuda.current_stream(dev).synchronize()   # the snapshot is complete when from_dense returns
+        return cls(bf16, i8, scales, index.dim, dev, index.row_offset)
+
+    @property
+    def n_rows(self) -> int:
+        return self._i8.shape[0]
+
+    @property
+    def rows_on_device(self) -> bool:
+        return self._rows.is_cuda
+
+    @property
+    def device_bytes(self) -> int:
+        """Bytes this index holds in device memory: int8 rows, scales and, with rows="device", the bf16 rows (shared
+        with the DenseIndex it came from)."""
+        b = self._i8.numel() + 4 * self._scales.numel()
+        if self._rows.is_cuda:
+            b += 2 * self._rows.shape[0] * self._rows.stride(0) if self._rows.shape[0] else 0
+        return b
+
+    # DenseIndex's conversion of host / device float queries to device bf16 [nq, dim_pad]
+    prepare_queries = DenseIndex.prepare_queries
+
+    def search_device(self, queries: torch.Tensor, k: int, candidates: Optional[int] = None,
+                      stream: Optional[torch.cuda.Stream] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Top k of a device bf16 [nq, dim_pad] query block: (ids int64 [nq, k], scores fp32 [nq, k]) on the device.
+        Scores are the exact fp32 dots of the rescore (descending, ties by ascending id); -1 / -inf where fewer than
+        k rows exist.  candidates (default min(128, 4 k)) rows per query come from the int8 scan."""
+        if candidates is None:
+            candidates = min(MAX_K, 4 * k)
+        if not (1 <= k <= candidates <= MAX_K):
+            raise ValueError(f"need 1 <= k <= candidates <= {MAX_K} (k={k}, candidates={candidates})")
+        if queries.dtype != torch.bfloat16 or queries.dim() != 2 or queries.shape[1] != self.dim_pad or not queries.is_cuda:
+            raise ValueError(f"queries must be device bf16 [nq, {self.dim_pad}]")
+        queries = queries.contiguous()
+        nq = queries.shape[0]
+        n = self.n_rows
+        lib = _native.load()
+        dev = self.device
+        with torch.cuda.device(dev):
+            st = stream if stream is not None else torch.cuda.current_stream(dev)
+            with torch.cuda.stream(st):
+                q8, qs = quantize_rows(queries, self.dim8, st)
+                c_ids = torch.empty((nq, candidates), dtype=torch.int64, device=dev)
+                c_sc = torch.empty((nq, candidates), dtype=torch.float32, device=dev)
+                ws_bytes = lib.crag_search_workspace_bytes(nq, candidates)
+                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+                rc = lib.crag_search_topk_i8(self._i8.data_ptr() if n else 0, self._scales.data_ptr() if n else 0, n,
+                                             self.dim8, self.dim8, self.row_offset, q8.data_ptr(), qs.data_ptr(), nq,
+                                             candidates, c_ids.data_ptr(), c_sc.data_ptr(), 0, ws.data_ptr(), ws_bytes,
+                                             st.cuda_stream)
+                _native.check(rc, "crag_search_topk_i8")
+                ids = torch.empty((nq, k), dtype=torch.int64, device=dev)
+                scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
+                rc = lib.crag_rescore_topk(self._rows.data_ptr() if n else 0, n, self.dim_pad,
+                                           self._rows.stride(0) if n else self.dim_pad, self.row_offset,
+                                           queries.data_ptr(), nq, c_ids.data_ptr(), candidates, k, ids.data_ptr(),
+                                           scores.data_ptr(), st.cuda_stream)
+                _native.check(rc, "crag_rescore_topk")
+        return ids, scores
+
+    def search(self, queries, k: int, candidates: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """Host entry point: what DenseIndex.prepare_queries accepts in, numpy (ids int64 [nq, k], scores fp32
+        [nq, k]) out."""
+        ids, scores = self.search_device(self.prepare_queries(queries), k, candidates)
+        return ids.cpu().numpy(), scores.cpu().numpy()

@@ -107,6 +107,41 @@ CRAG_API int crag_search_topk_after(const void* corpus, int64_t n_rows, int dim,
                                     int64_t* out_ids, float* out_scores, float* out_minmax, uint64_t* last_keys,
                                     void* workspace, size_t workspace_bytes, crag_stream_t stream);
 
+/* ------------------------------------------------------------------ int8 shards
+ * A shard stored as int8 rows with one fp32 scale per row: half the bytes per scan pass of the bf16 shard.  A search
+ * is crag_search_topk_i8 for k' candidates (k' <= 128) followed by crag_rescore_topk, which recomputes each candidate's
+ * score exactly from its bf16 row and keeps the best k.  The bf16 rows are read for the candidates only, so they may
+ * stay in page-locked host memory.  Semantics in DESIGN.md section 3e.
+ *
+ * crag_quantize_rows_i8: bf16 [n_rows, dim] rows (row stride row_stride elements, 1 <= dim <= 1024) ->
+ *   out_i8  device int8 [n_rows, out_stride], dim8 = ceil(dim / 128) * 128 columns written, zero padded;
+ *           out_stride >= dim8 and a multiple of 16, 16-B aligned
+ *   out_scales device fp32 [n_rows]:  s = amax / 127,  x^ = clamp(rint(x / s), -127, 127) (half to even), s = 0 for a
+ *           zero row.  Queries are quantised by the same call.  Rows must be finite. */
+CRAG_API int crag_quantize_rows_i8(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, void* out_i8,
+                                   int64_t out_stride, float* out_scales, crag_stream_t stream);
+/* crag_search_topk_i8: the top k (S1 descending, ties by ascending row) of
+ *   S1 = float(sum_i q^_i x^_i) * (s_q * s_row)   (exact s32 sum; fp32 products rounded to nearest)
+ * over an int8 shard [n_rows, dim8] (dim8 a multiple of 128, <= 1024; row_stride >= dim8 elements, a multiple of 16)
+ * with row_scales fp32 [n_rows], for queries_i8 int8 [nq, dim8] dense with query_scales fp32 [nq].  Outputs, (min, max)
+ * (over the shard's S1), row_offset and workspace (crag_search_workspace_bytes(nq, k)) as crag_search_topk. */
+CRAG_API int crag_search_topk_i8(const void* corpus_i8, const float* row_scales, int64_t n_rows, int dim8,
+                                 int64_t row_stride, int64_t row_offset, const void* queries_i8,
+                                 const float* query_scales, int nq, int k, int64_t* out_ids, float* out_scores,
+                                 float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream);
+/* crag_rescore_topk: per query, the top k (1 <= k <= n_cand <= 128) of its n_cand candidates cand_ids (device int64
+ * [nq, n_cand], global ids) by the fp32 dot of the bf16 row and the bf16 query, summed in the pinned order of DESIGN.md
+ * section 3e; ties by ascending row; -1 / -inf past the valid candidates.  An id outside [row_offset, row_offset +
+ * n_rows) is no candidate (as -1) and its row is never read.
+ *   rows_bf16     bf16 [n_rows, row_stride] in device memory or page-locked host memory (unified addressing);
+ *                 pageable host memory is refused with CRAG_ERR_INVALID before any launch.  16-B aligned,
+ *                 row_stride >= dim and a multiple of 8.
+ *   queries_bf16  device bf16 [nq, dim] dense, dim a multiple of 8 in [8, 1024], 16-B aligned
+ *   out_ids / out_scores  device int64 / fp32 [nq, k] */
+CRAG_API int crag_rescore_topk(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, int64_t row_offset,
+                               const void* queries_bf16, int nq, const int64_t* cand_ids, int n_cand, int k,
+                               int64_t* out_ids, float* out_scores, crag_stream_t stream);
+
 /* Exact top-k for large k and/or many queries: per chunk of queries one wgmma GEMM writes the fp32 score block
  * [q_chunk, round_up(n_rows, 4)] into the workspace, then one CTA per query radix-selects its k best.
  * Same argument rules and the same output contract as crag_search_topk (score desc, ties by ascending row, -1/-inf
