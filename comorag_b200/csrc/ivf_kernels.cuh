@@ -5,11 +5,9 @@
 #include <stdint.h>
 #include <cuda_runtime.h>
 
-#include "pool_floor.cuh"   // kNQ
+#include "pool_floor.cuh"   // kNQ, kTileRows
 
 namespace crag {
-
-constexpr int kTileRows = 128;  // corpus rows per tile (two wgmma M = 64 halves)
 
 // Builds one IVF pass's plan on the device (single CTA): which queries probe which list, their coarse terms, and the
 // work-list of the probed lists' tiles.  probed_ids / probed_scores are the coarse top-nprobe of each query

@@ -10,6 +10,7 @@
 namespace crag {
 
 constexpr int kNQ = 32;         // wgmma N: queries per pass
+constexpr int kTileRows = 128;  // corpus rows per tile (two wgmma M = 64 halves)
 
 // Pooled admission floor.  Every CTA publishes its current best kPoolM KEYS per query (after each flush of that
 // query's candidate buffer) in pool[cta][m][q] (packed u64 keys, 0 = nothing yet; query-contiguous so a warp reads

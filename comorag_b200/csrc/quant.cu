@@ -1,7 +1,43 @@
 // Int8 corpus shards: C entries of the quantiser and of the exact bf16 rescore (quant_kernels.cuh).  The int8 scan
-// between them, crag_search_topk_i8, is the I8 variant of the shard scan in search.cu.
+// between them, crag_search_topk_i8, is the I8 variant of the shard scan in search.cu.  The int8 IVF search
+// (crag_ivf_search_i8, search.cu) launches its rescore through launch_ivf_rescore here, so that the rescore kernels
+// have one translation unit.
 #include "common.cuh"
 #include "quant_kernels.cuh"
+
+namespace crag {
+
+// The rows may be device memory or page-locked host memory reached through unified addressing.  A kernel that
+// dereferences pageable host memory faults, so anything else is refused here, before a launch.
+int device_readable(const void* p, const void** out, const char* who) {
+  cudaPointerAttributes attr;
+  const cudaError_t e = cudaPointerGetAttributes(&attr, p);
+  if (e != cudaSuccess) {
+    cudaGetLastError();   // the failed query must not surface at the caller's next cudaGetLastError
+    return fail(CRAG_ERR_INVALID, "%s: rows are not memory the device can read (%s)", who, cudaGetErrorString(e));
+  }
+  if (attr.type == cudaMemoryTypeHost) {
+    if (!attr.devicePointer) return fail(CRAG_ERR_INVALID, "%s: page-locked rows are not mapped into the device's address space", who);
+    *out = attr.devicePointer;
+  } else if (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged) {
+    return fail(CRAG_ERR_INVALID, "%s: rows must be device memory or page-locked host memory (pageable host memory given)", who);
+  } else {
+    *out = p;
+  }
+  return CRAG_OK;
+}
+
+int launch_ivf_rescore(const void* rows, int64_t n_rows, int dim, int64_t row_stride, const void* queries, int nq,
+                       const int64_t* cand, int n_cand, int k, const int32_t* list_tile_start, int nlist,
+                       const float* coarse, int64_t* out_ids, float* out_scores, cudaStream_t stream) {
+  ivf_rescore_topk_kernel<<<nq, kRescoreThreads, 0, stream>>>(
+      static_cast<const uint16_t*>(rows), n_rows, dim, row_stride, static_cast<const uint16_t*>(queries), cand, n_cand, k,
+      out_ids, out_scores, IvfListTerm{list_tile_start, nlist, coarse});
+  CRAG_CUDA_OK(cudaGetLastError());
+  return CRAG_OK;
+}
+
+}  // namespace crag
 
 using namespace crag;
 
@@ -31,22 +67,10 @@ extern "C" int crag_rescore_topk(const void* rows_bf16, int64_t n_rows, int dim,
   if (row_stride < dim || row_stride % 8 != 0) return fail(CRAG_ERR_INVALID, "rescore: row_stride must be >= dim and a multiple of 8");
   if (!queries_bf16 || !cand_ids || !out_ids || !out_scores || (n_rows > 0 && !rows_bf16)) return fail(CRAG_ERR_INVALID, "rescore: null pointer");
   if ((reinterpret_cast<uintptr_t>(rows_bf16) | reinterpret_cast<uintptr_t>(queries_bf16)) & 15) return fail(CRAG_ERR_INVALID, "rescore: rows/queries must be 16-byte aligned");
-  // The rows may be device memory or page-locked host memory reached through unified addressing.  A kernel that
-  // dereferences pageable host memory faults, so anything else is refused here, before a launch.
   const void* rows = rows_bf16;
   if (n_rows > 0) {
-    cudaPointerAttributes attr;
-    const cudaError_t e = cudaPointerGetAttributes(&attr, rows_bf16);
-    if (e != cudaSuccess) {
-      cudaGetLastError();   // the failed query must not surface at the caller's next cudaGetLastError
-      return fail(CRAG_ERR_INVALID, "rescore: rows are not memory the device can read (%s)", cudaGetErrorString(e));
-    }
-    if (attr.type == cudaMemoryTypeHost) {
-      if (!attr.devicePointer) return fail(CRAG_ERR_INVALID, "rescore: page-locked rows are not mapped into the device's address space");
-      rows = attr.devicePointer;
-    } else if (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged) {
-      return fail(CRAG_ERR_INVALID, "rescore: rows must be device memory or page-locked host memory (pageable host memory given)");
-    }
+    const int rc = device_readable(rows_bf16, &rows, "rescore");
+    if (rc != CRAG_OK) return rc;
   }
   rescore_topk_kernel<<<nq, kRescoreThreads, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint16_t*>(rows), n_rows, dim, row_stride, row_offset, static_cast<const uint16_t*>(queries_bf16),

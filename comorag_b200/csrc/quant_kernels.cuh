@@ -9,11 +9,17 @@
 //             is added to the lane's partial (rounded) in element order from 0.f; the partials are combined by an
 //             xor-shuffle tree over 16, 8, 4, 2, 1.  The result is the top k of the candidates by (score descending,
 //             row ascending), as make_key orders them.
+//   IVF       (crag_ivf_search_i8, DESIGN.md 7) the candidates are stored positions p of an IVF shard's padded residual
+//             array; p's list l is the one with list_tile_start[l] <= p / 128 < list_tile_start[l + 1], and its score
+//             is fadd(dot, coarse[l][q]) with the pass's coarse table (ivf_plan_kernel).
 #pragma once
 #include <math.h>
 #include <stdint.h>
 #include <cuda_runtime.h>
 
+#include <type_traits>
+
+#include "pool_floor.cuh"   // kNQ, kTileRows
 #include "topk.cuh"
 
 namespace crag {
@@ -74,14 +80,38 @@ __device__ __forceinline__ float dot_chunk(float partial, const uint4& a, const 
   return partial;
 }
 
-// One CTA per query.  rows: bf16 [n_rows, row_stride] (device or page-locked host memory), queries: bf16 [nq, dim]
-// dense, dim a multiple of 8, rows and queries 16-byte aligned.  cand_ids: int64 [nq, n_cand] global ids; an id outside
-// [row_offset, row_offset + n_rows) -- -1 among them -- is no candidate and its row is never read.  Writes the top k
-// (k <= n_cand <= 128) to out_ids / out_scores [nq, k], -1 / -inf past the valid candidates.
-__global__ void __launch_bounds__(kRescoreThreads)
-rescore_topk_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride, int64_t row_offset,
-                    const uint16_t* __restrict__ queries, const int64_t* __restrict__ cand_ids, int n_cand, int k,
-                    int64_t* __restrict__ out_ids, float* __restrict__ out_scores) {
+// The flat rescore passes NoListTerm; the IVF rescore passes the list layout and the coarse table of its 32-query pass.
+struct NoListTerm {};
+struct IvfListTerm {
+  const int32_t* list_tile_start;   // [nlist + 1]
+  int nlist;
+  const float* coarse;              // [nlist][kNQ]: coarse[l * kNQ + q] = q . c_l for the lists query q probes
+};
+
+// the list owning stored position p: the largest l with list_tile_start[l] <= p / kTileRows, which skips empty lists
+__device__ __forceinline__ int list_of_position(const int32_t* __restrict__ list_tile_start, int nlist, int64_t p) {
+  const int32_t tile = int32_t(p / kTileRows);
+  int lo = 0, hi = nlist - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(&list_tile_start[mid]) <= tile) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// The body of both rescore kernels; one CTA per query.  rows: bf16 [n_rows, row_stride] (device or page-locked host
+// memory), queries: bf16 [nq, dim] dense, dim a multiple of 8, rows and queries 16-byte aligned.  cand_ids: int64
+// [nq, n_cand] global ids; an id outside [row_offset, row_offset + n_rows) -- -1 among them -- is no candidate and its
+// row is never read.  Writes the top k (k <= n_cand <= 128) to out_ids / out_scores [nq, k], -1 / -inf past the valid
+// candidates.
+template <class ListTerm>
+__device__ __forceinline__ void rescore_topk_body(const uint16_t* __restrict__ rows, int64_t n_rows, int dim,
+                                                  int64_t row_stride, int64_t row_offset,
+                                                  const uint16_t* __restrict__ queries,
+                                                  const int64_t* __restrict__ cand_ids, int n_cand, int k,
+                                                  int64_t* __restrict__ out_ids, float* __restrict__ out_scores,
+                                                  const ListTerm& lists) {
   __shared__ uint64_t keys[kRescoreMaxCand];
   const int q = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint16_t* qv = queries + int64_t(q) * dim;
@@ -97,6 +127,10 @@ rescore_topk_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, 
         partial = dot_chunk(partial, *reinterpret_cast<const uint4*>(xr + ch * 8), __ldg(reinterpret_cast<const uint4*>(qv + ch * 8)));
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) partial = __fadd_rn(partial, __shfl_xor_sync(0xffffffffu, partial, o));
+      if constexpr (std::is_same<ListTerm, IvfListTerm>::value) {
+        const int l = list_of_position(lists.list_tile_start, lists.nlist, local);
+        partial = __fadd_rn(partial, __ldg(&lists.coarse[int64_t(l) * kNQ + q]));
+      }
       key = make_key(partial, uint32_t(local));
     }
     if (lane == 0) keys[c] = key;
@@ -116,6 +150,23 @@ rescore_topk_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, 
       out_scores[int64_t(q) * k + g] = v[j] ? key_score(v[j]) : -INFINITY;
     }
   }
+}
+
+// crag_rescore_topk: candidates are global row ids
+__global__ void __launch_bounds__(kRescoreThreads)
+rescore_topk_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride, int64_t row_offset,
+                    const uint16_t* __restrict__ queries, const int64_t* __restrict__ cand_ids, int n_cand, int k,
+                    int64_t* __restrict__ out_ids, float* __restrict__ out_scores) {
+  rescore_topk_body(rows, n_rows, dim, row_stride, row_offset, queries, cand_ids, n_cand, k, out_ids, out_scores, NoListTerm{});
+}
+
+// crag_ivf_search_i8, one 32-query pass: candidates are stored positions of the IVF shard (row_offset 0, n_rows =
+// its padded row count), each score gains its list's coarse term; out_ids are positions (ivf_map_ids_kernel follows)
+__global__ void __launch_bounds__(kRescoreThreads)
+ivf_rescore_topk_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride,
+                        const uint16_t* __restrict__ queries, const int64_t* __restrict__ cand_ids, int n_cand, int k,
+                        int64_t* __restrict__ out_ids, float* __restrict__ out_scores, const IvfListTerm lists) {
+  rescore_topk_body(rows, n_rows, dim, row_stride, int64_t(0), queries, cand_ids, n_cand, k, out_ids, out_scores, lists);
 }
 
 }  // namespace crag

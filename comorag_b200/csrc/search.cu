@@ -26,7 +26,8 @@
 // The shard is read exactly once from HBM: algorithmic bytes = n_rows*dim*2.
 // Variants of the same pipeline: IVF = true walks a work-list of probed tiles
 // (crag_ivf_search); SCORES = true stores every score (crag_search_scores) or
-// keeps each row's running argmax over centroid blocks (crag_ivf_assign).
+// keeps each row's running argmax over centroid blocks (crag_ivf_assign);
+// I8 = true scans int8 rows (crag_search_topk_i8, and with IVF crag_ivf_search_i8).
 // Around it in this file: the per-shard merge (merge_topk_kernel), the fused
 // finalize + NVLink exchange + global merge of the row-sharded index
 // (finalize_exchange_kernel), the C-ABI entry points, and crag_knn_topk -- exact
@@ -88,8 +89,15 @@ struct I8Args {
   const float* row_scales;     // [n_rows]
   const float* query_scales;   // [nq] of this pass
 };
+// The int8 IVF scan (IVF = I8 = true, crag_ivf_search_i8) walks the IVF work-list over int8 residuals: the select warps
+// see the IvfArgs base, the wgmma warpgroup the scales.
+struct I8IvfArgs : IvfArgs {
+  const float* row_scales;     // [n_rows_padded], 0 on padding rows
+  const float* query_scales;   // [nq] of this pass
+};
 template <bool IVF, bool SCORES, bool I8> struct ScanParam { using type = typename IvfParam<IVF, SCORES>::type; };
 template <> struct ScanParam<false, false, true> { using type = I8Args; };
+template <> struct ScanParam<true, false, true> { using type = I8IvfArgs; };
 
 template <int KLIST, int CAP, int STAGES, bool IVF = false, bool SCORES = false, bool I8 = false>
 __global__ void __launch_bounds__(kSearchThreads, 1)
@@ -97,7 +105,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
                    int n_rows, int num_kb, int nq, int k, const uint64_t* __restrict__ after_keys,
                    uint64_t* __restrict__ pool, uint32_t perm_mul, int perm_shift, uint64_t* __restrict__ part_keys,
                    float* __restrict__ part_minmax, const typename ScanParam<IVF, SCORES, I8>::type args) {
-  static_assert(!I8 || (!IVF && !SCORES), "the int8 scan is a flat top-k scan");
+  static_assert(!(I8 && SCORES), "the int8 scan is a top-k scan");
   // elements per 128-byte swizzle row: the producer's column step per k-block
   constexpr int kBlockElems = I8 ? 128 : kBlockK;
   using L = SearchLayout<KLIST, CAP, STAGES>;
@@ -186,7 +194,9 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
       // I8: the scales of this thread's 4 rows of the tile (0 past n_rows), fetched while the k-blocks stream in
       float r_scale[I8 ? 4 : 1];
       if constexpr (I8) {
-        const int row0 = order(tile) * kTileRows;
+        int row0;
+        if constexpr (IVF) row0 = __ldg(&args.work[tile].x);
+        else row0 = order(tile) * kTileRows;
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const int row = row0 + (i >> 1) * 64 + frag_row + (i & 1) * 8;
@@ -242,7 +252,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
   } else {
     // ================================================================== select
     SmemScoreTiles tiles{score_tiles, bar_tfull, bar_tempty};
-    if constexpr (I8) select_warps<KLIST, CAP, false, false>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, NoIvfArgs{}, warp, lane);
+    if constexpr (I8 && !IVF) select_warps<KLIST, CAP, false, false>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, NoIvfArgs{}, warp, lane);
     else select_warps<KLIST, CAP, IVF, SCORES>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, args, warp, lane);
   }
 }
@@ -287,12 +297,12 @@ int launch_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_row
 }
 
 // A top-k scan with the selector of k: 64-key lists and 6 stages up to k = 64, 128-key lists and 4 stages above.
-// I8Args selects the int8 scan.
+// I8Args / I8IvfArgs select the int8 scan.
 template <bool IVF, class Args>
 int launch_topk_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k,
                      int grid, const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift,
                      uint64_t* part_keys, float* part_minmax, const Args& args, cudaStream_t stream) {
-  constexpr bool I8 = std::is_same<Args, I8Args>::value;
+  constexpr bool I8 = std::is_same<Args, I8Args>::value || std::is_same<Args, I8IvfArgs>::value;
   if (k <= 64) return launch_scan<64, 64, 6, IVF, false, I8>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
   return launch_scan<128, 128, 4, IVF, false, I8>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
 }
@@ -472,6 +482,104 @@ extern "C" int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int
     if (rc != CRAG_OK) return rc;
     rc = finalize_parts(workspace, sp.grid, nqc, k, 0, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
                         out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, nullptr, sp, stream);
+    if (rc != CRAG_OK) return rc;
+    ivf_map_ids_kernel<<<(nqc * k + 255) / 256, 256, 0, stream>>>(out_ids + size_t(q0) * k, nqc * k, row_ids);
+    CRAG_CUDA_OK(cudaGetLastError());
+  }
+  return CRAG_OK;
+}
+
+// ------------------------------------------------------------------ IVF over int8 residuals
+// Per 32-query pass: the IVF plan, the int8 scan of the probed tiles for n_cand candidates (S1 + coarse term), their
+// merge into the workspace, the exact bf16 rescore with the coarse term of each candidate's list (quant.cu), and the
+// map of stored positions to original ids.  The coarse table the rescore reads is the plan's, rebuilt every pass.
+namespace crag {
+namespace {
+struct IvfI8Plan {
+  IvfPlan ivf;
+  size_t cand_ids_off, cand_scores_off, total;
+};
+IvfI8Plan plan_ivf_i8(int nlist, int64_t total_tiles, int n_cand) {
+  IvfI8Plan p;
+  p.ivf = plan_ivf(plan_search(n_cand), nlist, total_tiles);
+  p.cand_ids_off = p.ivf.total;
+  p.cand_scores_off = p.cand_ids_off + ((size_t(kNQ) * n_cand * 8 + 255) & ~size_t(255));
+  p.total = p.cand_scores_off + ((size_t(kNQ) * n_cand * 4 + 255) & ~size_t(255));
+  return p;
+}
+}  // namespace
+}  // namespace crag
+
+extern "C" size_t crag_ivf_i8_workspace_bytes(int nlist, int64_t total_tiles, int n_cand) {
+  if (nlist < 1 || total_tiles < 0 || n_cand < 1 || n_cand > 128) return 0;
+  return plan_ivf_i8(nlist, total_tiles, n_cand).total;
+}
+
+extern "C" int crag_ivf_search_i8(const void* residuals_i8, const float* row_scales, int dim8, int64_t row_stride_i8,
+                                  const void* residuals_bf16, int dim, int64_t row_stride, int64_t n_rows_padded,
+                                  const int32_t* list_tile_start, const int32_t* list_rows, int nlist,
+                                  int64_t total_tiles, const int64_t* row_ids, const void* queries_i8,
+                                  const float* query_scales, const void* queries_bf16, int nq,
+                                  const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand, int k,
+                                  int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                                  size_t workspace_bytes, crag_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (nlist < 1 || nlist > (1 << 20) || nprobe < 1 || nprobe > nlist) return fail(CRAG_ERR_INVALID, "ivf_i8: need 1 <= nprobe <= nlist <= 2^20 (nprobe=%d nlist=%d)", nprobe, nlist);
+  if (nq < 1 || k < 1 || n_cand < k || n_cand > 128) return fail(CRAG_ERR_INVALID, "ivf_i8: need nq >= 1 and 1 <= k <= n_cand <= 128 (nq=%d k=%d n_cand=%d)", nq, k, n_cand);
+  if (dim < 64 || dim > 1024 || dim % 64 != 0) return fail(CRAG_ERR_INVALID, "ivf_i8: dim must be a multiple of 64 in [64, 1024] (dim=%d)", dim);
+  if (dim8 != (dim + 127) / 128 * 128) return fail(CRAG_ERR_INVALID, "ivf_i8: dim8 must be dim rounded up to a multiple of 128 (dim=%d dim8=%d)", dim, dim8);
+  if (total_tiles < 1 || total_tiles * kTileRows != n_rows_padded || n_rows_padded >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "ivf_i8: need n_rows_padded (%lld) = total_tiles (%lld) * %d, non-empty and below 2^31", (long long)n_rows_padded, (long long)total_tiles, kTileRows);
+  if (row_stride_i8 < dim8 || row_stride_i8 % 16 != 0) return fail(CRAG_ERR_INVALID, "ivf_i8: row_stride_i8 must be >= dim8 and a multiple of 16");
+  if (row_stride < dim || row_stride % 8 != 0) return fail(CRAG_ERR_INVALID, "ivf_i8: row_stride must be >= dim and a multiple of 8");
+  if (!residuals_i8 || !row_scales || !residuals_bf16 || !list_tile_start || !list_rows || !row_ids || !queries_i8 ||
+      !query_scales || !queries_bf16 || !probed_ids || !probed_scores || !out_ids || !out_scores || !workspace) return fail(CRAG_ERR_INVALID, "ivf_i8: null pointer");
+  if ((reinterpret_cast<uintptr_t>(residuals_i8) | reinterpret_cast<uintptr_t>(queries_i8) | reinterpret_cast<uintptr_t>(residuals_bf16) |
+       reinterpret_cast<uintptr_t>(queries_bf16)) & 15) return fail(CRAG_ERR_INVALID, "ivf_i8: residuals and queries must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "ivf_i8: workspace must be 256-byte aligned");
+  const IvfI8Plan plan = plan_ivf_i8(nlist, total_tiles, n_cand);
+  if (workspace_bytes < plan.total) return fail(CRAG_ERR_WORKSPACE, "ivf_i8: workspace %zu < %zu bytes", workspace_bytes, plan.total);
+  const void* rows_bf16 = nullptr;   // the bf16 residuals may be page-locked host memory: refused before any launch if pageable
+  int rc = device_readable(residuals_bf16, &rows_bf16, "ivf_i8");
+  if (rc != CRAG_OK) return rc;
+  const SearchPlan sp = plan_search(n_cand);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  uint64_t* part_keys = reinterpret_cast<uint64_t*>(ws);
+  float* part_minmax = reinterpret_cast<float*>(ws + sp.keys_bytes);
+  int64_t* cand_ids = reinterpret_cast<int64_t*>(ws + plan.cand_ids_off);
+  float* cand_scores = reinterpret_cast<float*>(ws + plan.cand_scores_off);
+  I8IvfArgs args;
+  args.list_mask = reinterpret_cast<uint32_t*>(ws + plan.ivf.mask_off);
+  args.coarse = reinterpret_cast<float*>(ws + plan.ivf.coarse_off);
+  args.work = reinterpret_cast<int4*>(ws + plan.ivf.work_off);
+  args.n_work = reinterpret_cast<int*>(ws + plan.ivf.count_off);
+  args.row_scales = row_scales;
+  CUtensorMap tm_res;
+  rc = make_tmap_u8_2d(&tm_res, residuals_i8, uint64_t(n_rows_padded), uint64_t(dim8), uint64_t(row_stride_i8), kTileRows);
+  if (rc != CRAG_OK) return rc;
+  for (int q0 = 0; q0 < nq; q0 += kNQ) {
+    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
+    CUtensorMap tm_q;
+    rc = make_tmap_u8_2d(&tm_q, static_cast<const uint8_t*>(queries_i8) + size_t(q0) * dim8, uint64_t(nqc), uint64_t(dim8), uint64_t(dim8), kNQ);
+    if (rc != CRAG_OK) return rc;
+    ivf_plan_kernel<<<1, 1024, 0, stream>>>(probed_ids + size_t(q0) * nprobe, probed_scores + size_t(q0) * nprobe, nqc, nprobe,
+                                            nlist, list_tile_start, list_rows, const_cast<uint32_t*>(args.list_mask),
+                                            const_cast<float*>(args.coarse), const_cast<int4*>(args.work), const_cast<int*>(args.n_work));
+    CRAG_CUDA_OK(cudaGetLastError());
+    uint64_t* pool = nullptr;
+    if (sp.pool_bytes) {
+      pool = reinterpret_cast<uint64_t*>(ws + plan.ivf.pool_off);
+      CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, sp.pool_bytes, stream));
+    }
+    args.query_scales = query_scales + q0;
+    rc = launch_topk_scan<true>(tm_res, tm_q, int(n_rows_padded), dim8 / 128, nqc, n_cand, sp.grid, nullptr, pool, 0u, 0,
+                                part_keys, part_minmax, args, stream);
+    if (rc != CRAG_OK) return rc;
+    rc = finalize_parts(workspace, sp.grid, nqc, n_cand, 0, cand_ids, cand_scores,
+                        out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, nullptr, sp, stream);
+    if (rc != CRAG_OK) return rc;
+    rc = launch_ivf_rescore(rows_bf16, n_rows_padded, dim, row_stride, static_cast<const uint8_t*>(queries_bf16) + size_t(q0) * dim * 2,
+                            nqc, cand_ids, n_cand, k, list_tile_start, nlist, args.coarse, out_ids + size_t(q0) * k,
+                            out_scores + size_t(q0) * k, stream);
     if (rc != CRAG_OK) return rc;
     ivf_map_ids_kernel<<<(nqc * k + 255) / 256, 256, 0, stream>>>(out_ids + size_t(q0) * k, nqc * k, row_ids);
     CRAG_CUDA_OK(cudaGetLastError());

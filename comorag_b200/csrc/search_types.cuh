@@ -5,8 +5,8 @@
 #include <stdint.h>
 #include <cuda_runtime.h>
 
-#include "ivf_kernels.cuh"   // kTileRows
-#include "pool_floor.cuh"    // kNQ
+#include "ivf_kernels.cuh"
+#include "pool_floor.cuh"    // kNQ, kTileRows
 
 namespace crag {
 

@@ -15,7 +15,8 @@ every list padded to whole 128-row tiles so that a tile belongs to exactly one l
 
 Index BUILD: the assignment of rows to centroids (k-means iterations and the final pass) is crag_ivf_assign -- the scan
 kernel with the rows as corpus and the centroid table as its query blocks; the centroid update and the counting sort
-by list are torch index arithmetic (bookkeeping).  SEARCH is crag_ivf_search.
+by list are torch index arithmetic (bookkeeping).  SEARCH is crag_ivf_search, or crag_ivf_search_i8 over an int8
+snapshot of the residuals (QuantizedIVF).
 """
 from __future__ import annotations
 
@@ -195,13 +196,116 @@ class IVFIndex:
         return ids.cpu().numpy(), scores.cpu().numpy()
 
 
+class QuantizedIVF:
+    """Frozen int8 snapshot of an IVFIndex (crag_ivf_search_i8; DESIGN.md section 7).  Every stored residual row is
+    quantised to int8 with one fp32 scale; a search scans the probed tiles' int8 residuals for `candidates` positions
+    per query (S1 = int8 dot * scales + coarse term) and rescores those exactly from their bf16 residuals
+    (S2 = pinned-order fp32 dot + coarse term).  The fine pass reads dim8 + 4 bytes per probed stored row instead of
+    2 dim.  The bf16 residuals are read for the candidates only, so they may live in page-locked host memory."""
+
+    def __init__(self, ivf: IVFIndex, residuals_bf16: torch.Tensor, residuals_i8: torch.Tensor, scales: torch.Tensor):
+        self.device, self.dim, self.nlist, self.n_rows = ivf.device, ivf.dim, ivf.nlist, ivf.n_rows
+        self.centroids = ivf.centroids
+        self.row_ids, self.list_tile_start, self.list_rows = ivf.row_ids, ivf.list_tile_start, ivf.list_rows
+        self.total_tiles = ivf.total_tiles
+        self._rows = residuals_bf16     # bf16 [total_tiles * 128, dim], on the device or in page-locked host memory
+        self._i8 = residuals_i8         # int8 [total_tiles * 128, dim8], device
+        self._scales = scales           # fp32 [total_tiles * 128], device; 0 on padding rows
+        self.dim8 = residuals_i8.shape[1]
+        self._lib = _native.load()
+
+    @classmethod
+    def from_ivf(cls, ivf: IVFIndex, residuals: str = "device") -> "QuantizedIVF":
+        """Quantise `ivf`'s stored residuals.  residuals="device" shares the IVFIndex's bf16 residual buffer;
+        residuals="host" copies it into page-locked host memory."""
+        from .quantized import _dim8, quantize_rows
+        if residuals not in ("device", "host"):
+            raise ValueError('residuals must be "device" or "host"')
+        bf16 = ivf.residuals
+        i8, scales = quantize_rows(bf16, _dim8(ivf.dim))
+        if residuals == "host":
+            host = torch.empty(tuple(bf16.shape), dtype=torch.bfloat16, pin_memory=True)
+            host.copy_(bf16)
+            bf16 = host
+        with torch.cuda.device(ivf.device):
+            torch.cuda.current_stream(ivf.device).synchronize()   # the snapshot is complete when from_ivf returns
+        return cls(ivf, bf16, i8, scales)
+
+    @property
+    def residuals_on_device(self) -> bool:
+        return self._rows.is_cuda
+
+    @property
+    def device_bytes(self) -> int:
+        """Bytes of the fine index in device memory: int8 residuals, their scales and, with residuals="device", the
+        bf16 residuals (shared with the IVFIndex).  The centroid table, row_ids and list tables are not counted."""
+        b = self._i8.numel() + 4 * self._scales.numel()
+        if self._rows.is_cuda:
+            b += 2 * self._rows.shape[0] * self._rows.stride(0) if self._rows.shape[0] else 0
+        return b
+
+    def search_device(self, queries_bf16: torch.Tensor, nprobe: int, k: int, candidates: Optional[int] = None,
+                      stream: Optional[torch.cuda.Stream] = None, probed: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
+        """bf16 [nq, dim] on the device -> (ids int64 [nq, k], scores fp32 [nq, k], minmax fp32 [nq, 2],
+        (probed list ids int64 [nq, nprobe], their coarse scores fp32)), as IVFIndex.search_device.  Scores are the
+        exact S2 values; minmax is (min, max) of the int8 stage's S1 over the probed rows.  candidates (default
+        min(128, 4 k)) positions per query come from the int8 scan; 1 <= k <= candidates <= 128."""
+        if candidates is None:
+            candidates = min(MAX_K, 4 * k)
+        if not 1 <= k <= candidates <= MAX_K:
+            raise ValueError(f"need 1 <= k <= candidates <= {MAX_K} (k={k}, candidates={candidates})")
+        if not 1 <= nprobe <= min(MAX_K, self.nlist):
+            raise ValueError(f"nprobe must be in [1, {min(MAX_K, self.nlist)}]")
+        if (queries_bf16.dtype != torch.bfloat16 or queries_bf16.dim() != 2 or queries_bf16.shape[1] != self.dim
+                or queries_bf16.device != self.device):
+            raise ValueError(f"queries must be bf16 [nq, {self.dim}] on {self.device}")
+        from .quantized import quantize_rows
+        q = queries_bf16.contiguous()
+        nq, dev = q.shape[0], self.device
+        with torch.cuda.device(dev):
+            st = stream if stream is not None else torch.cuda.current_stream(dev)
+            with torch.cuda.stream(st):
+                if probed is None:
+                    p_ids, p_scores, _ = self.centroids.search_device(q, nprobe, stream=st)
+                else:
+                    p_ids, p_scores = (t.contiguous() for t in probed)
+                    if (p_ids.dtype != torch.int64 or p_scores.dtype != torch.float32 or
+                            tuple(p_ids.shape) != (nq, nprobe) or tuple(p_scores.shape) != (nq, nprobe)):
+                        raise ValueError(f"probed must be (int64 [nq, {nprobe}], fp32 [nq, {nprobe}])")
+                q8, qs = quantize_rows(q, self.dim8, st)
+                ids = torch.empty((nq, k), dtype=torch.int64, device=dev)
+                scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
+                minmax = torch.empty((nq, 2), dtype=torch.float32, device=dev)
+                ws_bytes = self._lib.crag_ivf_i8_workspace_bytes(self.nlist, self.total_tiles, candidates)
+                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+                rc = self._lib.crag_ivf_search_i8(
+                    self._i8.data_ptr(), self._scales.data_ptr(), self.dim8, self._i8.stride(0),
+                    self._rows.data_ptr(), self.dim, self._rows.stride(0), self._rows.shape[0],
+                    self.list_tile_start.data_ptr(), self.list_rows.data_ptr(), self.nlist, self.total_tiles,
+                    self.row_ids.data_ptr(), q8.data_ptr(), qs.data_ptr(), q.data_ptr(), nq,
+                    p_ids.data_ptr(), p_scores.data_ptr(), nprobe, candidates, k,
+                    ids.data_ptr(), scores.data_ptr(), minmax.data_ptr(), ws.data_ptr(), ws_bytes, st.cuda_stream)
+                _native.check(rc, "crag_ivf_search_i8")
+        return ids, scores, minmax, (p_ids, p_scores)
+
+    def search(self, queries, nprobe: int, k: int, candidates: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """Host float [nq, dim] -> (ids int64 [nq, k], scores fp32 [nq, k]) as numpy."""
+        q = torch.as_tensor(queries)
+        if q.dim() == 1:
+            q = q[None, :]
+        q = q.to(self.device, non_blocking=True).to(torch.bfloat16)
+        ids, scores, _, _ = self.search_device(q, nprobe, k, candidates)
+        return ids.cpu().numpy(), scores.cpu().numpy()
+
+
 class ShardedIVF:
     """One rank's handle on a row-sharded IVF index (BASELINE config 4 on the GPUs of one box): every rank holds the
     SAME centroid table and the residual lists of its own rows, so all ranks probe the same lists; each searches its
     shard, ONE all-gather of the packed (ids, scores, min/max) records and the merge kernel give every rank the
     global answer -- the exchange step of the flat row-sharded index (dist.ShardedIndex), unchanged."""
 
-    def __init__(self, local: IVFIndex, group=None):
+    def __init__(self, local, group=None):
+        """`local`: this rank's IVFIndex or QuantizedIVF."""
         import torch.distributed as dist
         self.local, self.group = local, group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1

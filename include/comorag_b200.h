@@ -304,6 +304,31 @@ CRAG_API int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int d
                              int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
                              size_t workspace_bytes, crag_stream_t stream);
 
+/* IVF over int8 residuals: crag_ivf_search's shard layout with every stored residual row also quantised by
+ * crag_quantize_rows_i8 (padding rows are zero: scale 0).  Per block of 32 queries, in one call (the coarse table the
+ * rescore needs lives in the workspace and is rebuilt for every block): the IVF plan; an int8 scan of the probed tiles
+ * keeping the top n_cand stored positions by
+ *   S1 = float(sum_i q^_i r^_i) * (s_q * s_row) + (q . c_list)        (fp32 ops rounded to nearest, in this order)
+ * ties by ascending position; then, per candidate, S2 = dot + (q . c_list) with dot the fp32 dot of the bf16 residual
+ * and the bf16 query in crag_rescore_topk's pinned order; the top k by (S2 descending, position ascending), mapped to
+ * original ids through row_ids.  -1 / -inf past the valid candidates; out_minmax (may be NULL) is (min, max) of S1
+ * over the probed rows.  Semantics in DESIGN.md section 7.
+ *   residuals_i8  device int8 [n_rows_padded, row_stride_i8], dim8 = ceil(dim / 128) * 128 columns, row_scales fp32
+ *   residuals_bf16  bf16 [n_rows_padded, row_stride], device or page-locked host memory (pageable: CRAG_ERR_INVALID
+ *                 before any launch); dim a multiple of 64 in [64, 1024]
+ *   queries_i8 / query_scales  device int8 [nq, dim8] dense / fp32 [nq]; queries_bf16 device bf16 [nq, dim] dense
+ *   list layout, row_ids, probed_ids / probed_scores, nprobe as crag_ivf_search; 1 <= k <= n_cand <= 128.
+ * workspace >= crag_ivf_i8_workspace_bytes(nlist, total_tiles, n_cand), 256-byte aligned. */
+CRAG_API size_t crag_ivf_i8_workspace_bytes(int nlist, int64_t total_tiles, int n_cand);
+CRAG_API int crag_ivf_search_i8(const void* residuals_i8, const float* row_scales, int dim8, int64_t row_stride_i8,
+                                const void* residuals_bf16, int dim, int64_t row_stride, int64_t n_rows_padded,
+                                const int32_t* list_tile_start, const int32_t* list_rows, int nlist,
+                                int64_t total_tiles, const int64_t* row_ids, const void* queries_i8,
+                                const float* query_scales, const void* queries_bf16, int nq,
+                                const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand, int k,
+                                int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                                size_t workspace_bytes, crag_stream_t stream);
+
 /* IVF build, assignment step: best_id[r] = argmax_l bf16(row r) . bf16(centroid l) (fp32 accumulation on the tensor
  * cores, ties to the smaller l), best_score[r] = that inner product.  rows device bf16 [n_rows, dim] (row_stride
  * elements), centroids device bf16 [nlist, dim] contiguous; outputs device fp32 / int32 [n_rows].  nlist / 32 passes of
