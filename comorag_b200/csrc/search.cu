@@ -24,10 +24,9 @@
 //            The admission threshold is the better of the CTA's own k-th key
 //            and a floor pooled over ALL CTAs (kPoolM below).
 // The shard is read exactly once from HBM: algorithmic bytes = n_rows*dim*2.
-// Variants of the same pipeline: IVF = true walks a work-list of probed tiles
-// (crag_ivf_search); SCORES = true stores every score (crag_search_scores) or
-// keeps each row's running argmax over centroid blocks (crag_ivf_assign);
-// I8 = true scans int8 rows (crag_search_topk_i8, and with IVF crag_ivf_search_i8).
+// Variants of the same pipeline, named by the kernel's argument struct: IvfArgs walks a work-list of probed tiles
+// (crag_ivf_search); ScoreArgs stores every score (crag_search_scores) or keeps each row's running argmax over centroid
+// blocks (crag_ivf_assign); I8Args scans int8 rows (crag_search_topk_i8), I8IvfArgs int8 IVF lists (crag_ivf_search_i8).
 // Around it in this file: the per-shard merge (merge_topk_kernel), the fused
 // finalize + NVLink exchange + global merge of the row-sharded index
 // (finalize_exchange_kernel), the C-ABI entry points, and crag_knn_topk -- exact
@@ -81,31 +80,25 @@ struct SmemScoreTiles {
   }
 };
 
-// Int8 variant of the flat top-k scan (I8 = true, crag_search_topk_i8): the shard and the query block are int8 with one
+// Int8 variant of the flat top-k scan (I8Args, crag_search_topk_i8): the shard and the query block are int8 with one
 // fp32 scale per row / query (quant_kernels.cuh).  A 128-byte swizzle row holds 128 int8 instead of 64 bf16, so boxes,
 // stages, descriptors and score tiles keep their byte sizes; the warpgroup issues m64n32k32.s32.s8.s8 and its epilogue
 // writes S1 = float(acc) * (s_q * s_row) to the score tile, which the select warps rank as they rank bf16 scores.
 struct I8Args {
-  const float* row_scales;     // [n_rows]
+  const float* row_scales;     // [n_rows], 0 on IVF padding rows
   const float* query_scales;   // [nq] of this pass
 };
-// The int8 IVF scan (IVF = I8 = true, crag_ivf_search_i8) walks the IVF work-list over int8 residuals: the select warps
-// see the IvfArgs base, the wgmma warpgroup the scales.
-struct I8IvfArgs : IvfArgs {
-  const float* row_scales;     // [n_rows_padded], 0 on padding rows
-  const float* query_scales;   // [nq] of this pass
-};
-template <bool IVF, bool SCORES, bool I8> struct ScanParam { using type = typename IvfParam<IVF, SCORES>::type; };
-template <> struct ScanParam<false, false, true> { using type = I8Args; };
-template <> struct ScanParam<true, false, true> { using type = I8IvfArgs; };
+// The int8 IVF scan (crag_ivf_search_i8): the select warps read the IvfArgs part, the wgmma warpgroup the scales.
+struct I8IvfArgs : IvfArgs, I8Args {};
+template <class Args> constexpr bool kI8Scan = std::is_base_of<I8Args, Args>::value;
 
-template <int KLIST, int CAP, int STAGES, bool IVF = false, bool SCORES = false, bool I8 = false>
+template <int KLIST, int CAP, int STAGES, class Args>
 __global__ void __launch_bounds__(kSearchThreads, 1)
 search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_constant__ CUtensorMap tm_q,
                    int n_rows, int num_kb, int nq, int k, const uint64_t* __restrict__ after_keys,
                    uint64_t* __restrict__ pool, uint32_t perm_mul, int perm_shift, uint64_t* __restrict__ part_keys,
-                   float* __restrict__ part_minmax, const typename ScanParam<IVF, SCORES, I8>::type args) {
-  static_assert(!(I8 && SCORES), "the int8 scan is a top-k scan");
+                   float* __restrict__ part_minmax, const Args args) {
+  constexpr bool IVF = kIvfScan<Args>, SCORES = kScoreScan<Args>, I8 = kI8Scan<Args>;
   // elements per 128-byte swizzle row: the producer's column step per k-block
   constexpr int kBlockElems = I8 ? 128 : kBlockK;
   using L = SearchLayout<KLIST, CAP, STAGES>;
@@ -252,8 +245,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
   } else {
     // ================================================================== select
     SmemScoreTiles tiles{score_tiles, bar_tfull, bar_tempty};
-    if constexpr (I8 && !IVF) select_warps<KLIST, CAP, false, false>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, NoIvfArgs{}, warp, lane);
-    else select_warps<KLIST, CAP, IVF, SCORES>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, args, warp, lane);
+    select_warps<KLIST, CAP, IVF, SCORES>(sel, tiles, order, num_tiles, n_rows, nq, k, after_keys, pool, part_keys, part_minmax, args, warp, lane);
   }
 }
 
@@ -278,12 +270,12 @@ SearchPlan plan_search(int k) {
 }
 
 // One launch of the scan.  The dynamic shared-memory limit is raised once per instantiation and device.
-template <int KLIST, int CAP, int STAGES, bool IVF, bool SCORES, bool I8 = false>
+template <int KLIST, int CAP, int STAGES, class Args>
 int launch_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k, int grid,
                 const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift, uint64_t* part_keys,
-                float* part_minmax, const typename ScanParam<IVF, SCORES, I8>::type& args, cudaStream_t stream) {
+                float* part_minmax, const Args& args, cudaStream_t stream) {
   constexpr size_t smem = SearchLayout<KLIST, CAP, STAGES>::smem_bytes();
-  auto kern = search_topk_kernel<KLIST, CAP, STAGES, IVF, SCORES, I8>;
+  auto kern = search_topk_kernel<KLIST, CAP, STAGES, Args>;
   static bool attr_set[64] = {};
   int dev = 0;
   CRAG_CUDA_OK(cudaGetDevice(&dev));
@@ -297,14 +289,12 @@ int launch_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_row
 }
 
 // A top-k scan with the selector of k: 64-key lists and 6 stages up to k = 64, 128-key lists and 4 stages above.
-// I8Args / I8IvfArgs select the int8 scan.
-template <bool IVF, class Args>
+template <class Args>
 int launch_topk_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k,
                      int grid, const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift,
                      uint64_t* part_keys, float* part_minmax, const Args& args, cudaStream_t stream) {
-  constexpr bool I8 = std::is_same<Args, I8Args>::value || std::is_same<Args, I8IvfArgs>::value;
-  if (k <= 64) return launch_scan<64, 64, 6, IVF, false, I8>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
-  return launch_scan<128, 128, 4, IVF, false, I8>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+  if (k <= 64) return launch_scan<64, 64, 6>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+  return launch_scan<128, 128, 4>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
 }
 
 // The merge kernels' list size for k (32, 64 or 128), passed to `launch` as a std::integral_constant.
@@ -315,9 +305,54 @@ void with_merge_tier(int k, Launch launch) {
   else launch(std::integral_constant<int, 128>{});
 }
 
-// tensor map of queries q0 .. q0 + nqc - 1 (nqc <= 32) of a dense [nq, dim] bf16 array
-int make_query_tmap(CUtensorMap* tm, const void* queries, int q0, int nqc, int dim) {
-  return make_tmap_bf16_2d(tm, static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, uint64_t(nqc), uint64_t(dim), uint64_t(dim) * 2, kNQ);
+// the scan arguments of the pass over queries q0 .. q0 + 31: the int8 scans read the scales of that pass's queries
+template <class Args>
+Args pass_args(Args args, int q0) {
+  if constexpr (kI8Scan<Args>) args.query_scales += q0;
+  return args;
+}
+
+// A scan operand: `rows` rows of `width` elements, `stride` elements apart; `name` heads its error messages.
+enum Elem { kS8 = 1, kBf16 = 2 };   // bytes per element
+struct Operand {
+  const void* ptr;
+  int64_t rows;
+  int width;
+  int64_t stride;
+  Elem elem;
+  const char* name;
+  Operand rows_from(int64_t r0, int64_t n) const { return {static_cast<const uint8_t*>(ptr) + r0 * stride * elem, n, width, stride, elem, name}; }
+  int num_kb() const { return width * elem / 128; }   // 128-byte swizzle rows per row
+};
+
+// The scan's rules for an operand, in bytes: 1 to 1024 elements per row in whole 128-byte swizzle rows (bf16 dim % 64,
+// int8 dim % 128), a row stride of whole 16 bytes, a 16-byte aligned base and row indices that fit an int.
+int check_operand(const char* who, const Operand& op) {
+  if (op.width < 1 || op.width > 1024 || op.width * op.elem % 128 != 0) return fail(CRAG_ERR_INVALID, "%s: %s dim must be a multiple of %d in [%d, 1024] (dim=%d)", who, op.name, 128 / op.elem, 128 / op.elem, op.width);
+  if (op.rows < 0 || op.rows >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "%s: %s n_rows out of range (%lld)", who, op.name, (long long)op.rows);
+  if (op.stride < op.width || op.stride * op.elem % 16 != 0) return fail(CRAG_ERR_INVALID, "%s: %s row stride must be >= dim and a multiple of %d", who, op.name, 16 / op.elem);
+  if (op.rows > 0 && !op.ptr) return fail(CRAG_ERR_INVALID, "%s: null %s pointer", who, op.name);
+  if (reinterpret_cast<uintptr_t>(op.ptr) & 15) return fail(CRAG_ERR_INVALID, "%s: %s must be 16-byte aligned", who, op.name);
+  return CRAG_OK;
+}
+
+// nq and k, the shard and query operands of a scan, and a 256-byte aligned workspace of at least `need` bytes
+int check_scan_args(const char* who, int nq, int k, int k_max, const Operand& corpus, const Operand& queries,
+                    const void* workspace, size_t workspace_bytes, size_t need) {
+  if (nq < 1 || k < 1 || k > k_max) return fail(CRAG_ERR_INVALID, "%s: need nq >= 1 and 1 <= k <= %d (nq=%d k=%d)", who, k_max, nq, k);
+  int rc = check_operand(who, corpus);
+  if (rc == CRAG_OK) rc = check_operand(who, queries);
+  if (rc != CRAG_OK) return rc;
+  if (!workspace) return fail(CRAG_ERR_INVALID, "%s: null workspace pointer", who);
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "%s: workspace must be 256-byte aligned", who);
+  if (workspace_bytes < need) return fail(CRAG_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes", who, workspace_bytes, need);
+  return CRAG_OK;
+}
+
+// TMA map of an operand in boxes of box_rows rows by one 128-byte swizzle row
+int make_tmap(CUtensorMap* tm, const Operand& op, uint32_t box_rows) {
+  if (op.elem == kS8) return make_tmap_u8_2d(tm, op.ptr, uint64_t(op.rows), uint64_t(op.width), uint64_t(op.stride), box_rows);
+  return make_tmap_bf16_2d(tm, op.ptr, uint64_t(op.rows), uint64_t(op.width), uint64_t(op.stride) * 2, box_rows);
 }
 
 }  // namespace
@@ -335,20 +370,6 @@ extern "C" size_t crag_search_workspace_bytes(int nq, int k) {
 namespace crag {
 namespace {
 
-int check_search_args(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride, const void* queries,
-                      int nq, int k, const void* workspace, size_t workspace_bytes, const SearchPlan& plan,
-                      int k_max = 128) {
-  if (nq < 1 || k < 1 || k > k_max) return fail(CRAG_ERR_INVALID, "search: need nq >= 1 and 1 <= k <= %d (nq=%d k=%d)", k_max, nq, k);
-  if (dim < 64 || dim > 1024 || dim % 64 != 0) return fail(CRAG_ERR_INVALID, "search: dim must be a multiple of 64 in [64, 1024] (dim=%d)", dim);
-  if (n_rows < 0 || n_rows >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "search: n_rows out of range (%lld)", (long long)n_rows);
-  if (corpus_row_stride < dim || corpus_row_stride % 8 != 0) return fail(CRAG_ERR_INVALID, "search: corpus_row_stride must be >= dim and a multiple of 8");
-  if (!queries || !workspace || (n_rows > 0 && !corpus)) return fail(CRAG_ERR_INVALID, "search: null pointer");
-  if ((reinterpret_cast<uintptr_t>(corpus) | reinterpret_cast<uintptr_t>(queries)) & 15) return fail(CRAG_ERR_INVALID, "search: corpus/queries must be 16-byte aligned");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "search: workspace must be 256-byte aligned");
-  if (workspace_bytes < plan.keys_bytes + plan.minmax_bytes) return fail(CRAG_ERR_WORKSPACE, "search: workspace %zu < %zu bytes", workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
-  return CRAG_OK;
-}
-
 inline int scan_grid(int64_t n_rows, const SearchPlan& plan) {
   const int num_tiles = int((n_rows + kTileRows - 1) / kTileRows);
   return num_tiles < plan.grid ? num_tiles : plan.grid;
@@ -357,38 +378,27 @@ inline int scan_grid(int64_t n_rows, const SearchPlan& plan) {
 // the flat scans permute groups of 2^kPermShift consecutive tiles (TileOrder)
 constexpr int kPermShift = 3;
 
-// one corpus pass for queries q0 .. q0 + nq - 1 (nq <= 32): per-CTA partial lists into the workspace.  With `i8` the
-// corpus and queries are int8 [*, dim] (dim a multiple of 128) with the scales of i8 (query scales from query 0 on).
-int scan_pass(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride, const void* queries, int q0,
-              int nq, int k, const uint64_t* after_keys, void* workspace, size_t workspace_bytes,
-              const SearchPlan& plan, cudaStream_t stream, const I8Args* i8 = nullptr) {
-  const int grid = scan_grid(n_rows, plan);
+// one corpus pass for the <= 32 queries of `queries`: per-CTA partial lists into the workspace
+template <class Args>
+int scan_pass(const Operand& corpus, const Operand& queries, int k, const uint64_t* after_keys, const Args& args,
+              void* workspace, size_t workspace_bytes, const SearchPlan& plan, cudaStream_t stream) {
+  const int grid = scan_grid(corpus.rows, plan);
   if (grid == 0) return CRAG_OK;
   uint64_t* part_keys = static_cast<uint64_t*>(workspace);
   float* part_minmax = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + plan.keys_bytes);
   // pooled floor: needs its table in the workspace and pays off once a CTA sees more than a couple of tiles
   uint64_t* pool = nullptr;
-  const int64_t num_tiles = (n_rows + kTileRows - 1) / kTileRows;
+  const int64_t num_tiles = (corpus.rows + kTileRows - 1) / kTileRows;
   if (plan.pool_bytes && workspace_bytes >= plan.keys_bytes + plan.minmax_bytes + plan.pool_bytes && num_tiles >= 4 * int64_t(grid)) {
     pool = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(workspace) + plan.keys_bytes + plan.minmax_bytes);
     CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, plan.pool_bytes, stream));
   }
   CUtensorMap tm_corpus, tm_q;
-  if (i8) {
-    int rc = make_tmap_u8_2d(&tm_corpus, corpus, uint64_t(n_rows), uint64_t(dim), uint64_t(corpus_row_stride), kTileRows);
-    if (rc != CRAG_OK) return rc;
-    rc = make_tmap_u8_2d(&tm_q, static_cast<const uint8_t*>(queries) + size_t(q0) * dim, uint64_t(nq), uint64_t(dim), uint64_t(dim), kNQ);
-    if (rc != CRAG_OK) return rc;
-    return launch_topk_scan<false>(tm_corpus, tm_q, int(n_rows), dim / 128, nq, k, grid, after_keys, pool,
-                                   perm_multiplier(num_tiles >> kPermShift), kPermShift, part_keys, part_minmax,
-                                   I8Args{i8->row_scales, i8->query_scales + q0}, stream);
-  }
-  int rc = make_tmap_bf16_2d(&tm_corpus, corpus, uint64_t(n_rows), uint64_t(dim), uint64_t(corpus_row_stride) * 2, kTileRows);
+  int rc = make_tmap(&tm_corpus, corpus, kTileRows);
+  if (rc == CRAG_OK) rc = make_tmap(&tm_q, queries, kNQ);
   if (rc != CRAG_OK) return rc;
-  rc = make_query_tmap(&tm_q, queries, q0, nq, dim);
-  if (rc != CRAG_OK) return rc;
-  return launch_topk_scan<false>(tm_corpus, tm_q, int(n_rows), dim / kBlockK, nq, k, grid, after_keys, pool,
-                                 perm_multiplier(num_tiles >> kPermShift), kPermShift, part_keys, part_minmax, NoIvfArgs{}, stream);
+  return launch_topk_scan(tm_corpus, tm_q, int(corpus.rows), corpus.num_kb(), int(queries.rows), k, grid, after_keys, pool,
+                          perm_multiplier(num_tiles >> kPermShift), kPermShift, part_keys, part_minmax, args, stream);
 }
 
 // merge the per-CTA partials of one pass into the final (ids, scores, minmax) of its <= 32 queries
@@ -405,10 +415,22 @@ int finalize_parts(const void* workspace, int grid, int nq, int k, int64_t row_o
   return CRAG_OK;
 }
 
-int finalize_pass(const void* workspace, int64_t n_rows, int nq, int k, int64_t row_offset, int64_t* out_ids,
-                  float* out_scores, float* out_minmax, uint64_t* last_keys, const SearchPlan& plan, cudaStream_t stream) {
-  return finalize_parts(workspace, scan_grid(n_rows, plan), nq, k, row_offset, out_ids, out_scores, out_minmax, last_keys,
-                        plan, stream);
+// every 32-query pass of a flat top-k scan: the scan, then the merge of its partials into the outputs
+template <class Args>
+int topk_passes(const Operand& corpus, const Operand& queries, int k, int64_t row_offset, const uint64_t* after_keys,
+                const Args& args, int64_t* out_ids, float* out_scores, float* out_minmax, uint64_t* last_keys,
+                void* workspace, size_t workspace_bytes, const SearchPlan& plan, cudaStream_t stream) {
+  const int nq = int(queries.rows);
+  for (int q0 = 0; q0 < nq; q0 += kNQ) {
+    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
+    int rc = scan_pass(corpus, queries.rows_from(q0, nqc), k, after_keys ? after_keys + q0 : nullptr, pass_args(args, q0),
+                       workspace, workspace_bytes, plan, stream);
+    if (rc == CRAG_OK)
+      rc = finalize_parts(workspace, scan_grid(corpus.rows, plan), nqc, k, row_offset, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
+                         out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, last_keys ? last_keys + q0 : nullptr, plan, stream);
+    if (rc != CRAG_OK) return rc;
+  }
+  return CRAG_OK;
 }
 
 // IVF workspace = the flat scan's per-CTA partials, then the per-pass plan
@@ -427,6 +449,100 @@ IvfPlan plan_ivf(const SearchPlan& sp, int nlist, int64_t total_tiles) {
   return p;
 }
 
+struct IvfI8Plan {
+  IvfPlan ivf;
+  size_t cand_ids_off, cand_scores_off, total;
+};
+IvfI8Plan plan_ivf_i8(int nlist, int64_t total_tiles, int n_cand) {
+  IvfI8Plan p;
+  p.ivf = plan_ivf(plan_search(n_cand), nlist, total_tiles);
+  p.cand_ids_off = p.ivf.total;
+  p.cand_scores_off = p.cand_ids_off + ((size_t(kNQ) * n_cand * 8 + 255) & ~size_t(255));
+  p.total = p.cand_scores_off + ((size_t(kNQ) * n_cand * 4 + 255) & ~size_t(255));
+  return p;
+}
+
+struct IvfLists {   // the list tables and probes of an IVF search, as crag_ivf_search takes them
+  const int32_t* tile_start;
+  const int32_t* rows;
+  int nlist;
+  int64_t total_tiles;
+  const int64_t* row_ids;
+  const int64_t* probed_ids;
+  const float* probed_scores;
+  int nprobe;
+};
+
+// the lists, the probes and the outputs of an IVF search over n_rows_padded stored rows in whole tiles
+int check_ivf_args(const char* who, const IvfLists& l, int64_t n_rows_padded, const int64_t* out_ids, const float* out_scores) {
+  if (l.nlist < 1 || l.nlist > (1 << 20) || l.nprobe < 1 || l.nprobe > l.nlist) return fail(CRAG_ERR_INVALID, "%s: need 1 <= nprobe <= nlist <= 2^20 (nprobe=%d nlist=%d)", who, l.nprobe, l.nlist);
+  if (l.total_tiles < 1 || l.total_tiles * kTileRows != n_rows_padded) return fail(CRAG_ERR_INVALID, "%s: need n_rows_padded (%lld) = total_tiles (%lld) * %d, non-empty", who, (long long)n_rows_padded, (long long)l.total_tiles, kTileRows);
+  if (!l.tile_start || !l.rows || !l.row_ids || !l.probed_ids || !l.probed_scores || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "%s: null pointer", who);
+  return CRAG_OK;
+}
+
+// crag_ivf_search_i8's exact rescore: bf16 residuals (device address) and queries, and the candidates' workspace buffers
+struct IvfRescore {
+  Operand rows, queries;
+  int64_t* cand_ids;
+  float* cand_scores;
+};
+
+// Every 32-query pass of an IVF search over the residuals `res`: the plan of the probed tiles, the scan for n_scan keys
+// per query, the merge of its partials, then the map of stored positions to original ids.  With `rescore` the merge
+// writes n_scan candidates, which the exact rescore (quant.cu) turns into the k results, with the plan's coarse terms.
+template <class Args>
+int ivf_passes(const Operand& res, const Operand& queries, Args args, const IvfLists& l, int n_scan, int k,
+               const IvfRescore* rescore, int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+               const IvfPlan& ip, const SearchPlan& sp, cudaStream_t stream) {
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  uint64_t* part_keys = reinterpret_cast<uint64_t*>(ws);
+  float* part_minmax = reinterpret_cast<float*>(ws + sp.keys_bytes);
+  uint32_t* list_mask = reinterpret_cast<uint32_t*>(ws + ip.mask_off);
+  float* coarse = reinterpret_cast<float*>(ws + ip.coarse_off);
+  int4* work = reinterpret_cast<int4*>(ws + ip.work_off);
+  int* n_work = reinterpret_cast<int*>(ws + ip.count_off);
+  static_cast<IvfArgs&>(args) = IvfArgs{work, n_work, list_mask, coarse};
+  CUtensorMap tm_res;
+  int rc = make_tmap(&tm_res, res, kTileRows);
+  if (rc != CRAG_OK) return rc;
+  const int nq = int(queries.rows);
+  for (int q0 = 0; q0 < nq; q0 += kNQ) {
+    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
+    CUtensorMap tm_q;
+    rc = make_tmap(&tm_q, queries.rows_from(q0, nqc), kNQ);
+    if (rc != CRAG_OK) return rc;
+    ivf_plan_kernel<<<1, 1024, 0, stream>>>(l.probed_ids + size_t(q0) * l.nprobe, l.probed_scores + size_t(q0) * l.nprobe, nqc,
+                                            l.nprobe, l.nlist, l.tile_start, l.rows, list_mask, coarse, work, n_work);
+    CRAG_CUDA_OK(cudaGetLastError());
+    // every CTA of the grid publishes a (possibly empty) partial list, so the merge always reads sp.grid parts
+    uint64_t* pool = nullptr;
+    if (sp.pool_bytes) {
+      pool = reinterpret_cast<uint64_t*>(ws + ip.pool_off);
+      CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, sp.pool_bytes, stream));
+    }
+    rc = launch_topk_scan(tm_res, tm_q, int(res.rows), res.num_kb(), nqc, n_scan, sp.grid, nullptr, pool, 0u, 0,
+                          part_keys, part_minmax, pass_args(args, q0), stream);
+    if (rc != CRAG_OK) return rc;
+    int64_t* ids = out_ids + size_t(q0) * k;
+    float* scores = out_scores + size_t(q0) * k;
+    float* minmax = out_minmax ? out_minmax + size_t(q0) * 2 : nullptr;
+    if (!rescore) {
+      rc = finalize_parts(workspace, sp.grid, nqc, k, 0, ids, scores, minmax, nullptr, sp, stream);
+    } else {
+      rc = finalize_parts(workspace, sp.grid, nqc, n_scan, 0, rescore->cand_ids, rescore->cand_scores, minmax, nullptr, sp, stream);
+      if (rc == CRAG_OK)
+        rc = launch_ivf_rescore(rescore->rows.ptr, rescore->rows.rows, rescore->rows.width, rescore->rows.stride,
+                                rescore->queries.rows_from(q0, nqc).ptr, nqc, rescore->cand_ids, n_scan, k, l.tile_start,
+                                l.nlist, coarse, ids, scores, stream);
+    }
+    if (rc != CRAG_OK) return rc;
+    ivf_map_ids_kernel<<<(nqc * k + 255) / 256, 256, 0, stream>>>(ids, nqc * k, l.row_ids);
+    CRAG_CUDA_OK(cudaGetLastError());
+  }
+  return CRAG_OK;
+}
+
 }  // namespace
 }  // namespace crag
 
@@ -440,76 +556,20 @@ extern "C" int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int
                                int64_t total_tiles, const int64_t* row_ids, const void* queries, int nq,
                                const int64_t* probed_ids, const float* probed_scores, int nprobe, int k,
                                int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
-                               size_t workspace_bytes, crag_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+                               size_t workspace_bytes, crag_stream_t stream) {
+  const Operand res{residuals, n_rows_padded, dim, row_stride, kBf16, "residuals"}, q{queries, nq, dim, dim, kBf16, "queries"};
+  const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
+  int rc = check_ivf_args("ivf", lists, n_rows_padded, out_ids, out_scores);
+  if (rc != CRAG_OK) return rc;
   const SearchPlan sp = plan_search(k >= 1 && k <= 128 ? k : 1);
-  if (nlist < 1 || nlist > (1 << 20) || nprobe < 1 || nprobe > nlist) return fail(CRAG_ERR_INVALID, "ivf: need 1 <= nprobe <= nlist <= 2^20 (nprobe=%d nlist=%d)", nprobe, nlist);
-  if (total_tiles < 0 || total_tiles * kTileRows != n_rows_padded) return fail(CRAG_ERR_INVALID, "ivf: n_rows_padded (%lld) must be total_tiles (%lld) * %d", (long long)n_rows_padded, (long long)total_tiles, kTileRows);
   const IvfPlan ip = plan_ivf(sp, nlist, total_tiles);
-  int rc = check_search_args(residuals, n_rows_padded, dim, row_stride, queries, nq, k, workspace, workspace_bytes, sp);
+  rc = check_scan_args("ivf", nq, k, 128, res, q, workspace, workspace_bytes, ip.total);
   if (rc != CRAG_OK) return rc;
-  if (workspace_bytes < ip.total) return fail(CRAG_ERR_WORKSPACE, "ivf: workspace %zu < %zu bytes", workspace_bytes, ip.total);
-  if (!list_tile_start || !list_rows || !row_ids || !probed_ids || !probed_scores || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "ivf: null pointer");
-  if (n_rows_padded == 0) return fail(CRAG_ERR_INVALID, "ivf: empty index");
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  uint64_t* part_keys = reinterpret_cast<uint64_t*>(ws);
-  float* part_minmax = reinterpret_cast<float*>(ws + sp.keys_bytes);
-  IvfArgs ivf;
-  ivf.list_mask = reinterpret_cast<uint32_t*>(ws + ip.mask_off);
-  ivf.coarse = reinterpret_cast<float*>(ws + ip.coarse_off);
-  ivf.work = reinterpret_cast<int4*>(ws + ip.work_off);
-  ivf.n_work = reinterpret_cast<int*>(ws + ip.count_off);
-  CUtensorMap tm_res;
-  rc = make_tmap_bf16_2d(&tm_res, residuals, uint64_t(n_rows_padded), uint64_t(dim), uint64_t(row_stride) * 2, kTileRows);
-  if (rc != CRAG_OK) return rc;
-  const int num_kb = dim / kBlockK;
-  for (int q0 = 0; q0 < nq; q0 += kNQ) {
-    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
-    CUtensorMap tm_q;
-    rc = make_query_tmap(&tm_q, queries, q0, nqc, dim);
-    if (rc != CRAG_OK) return rc;
-    ivf_plan_kernel<<<1, 1024, 0, stream>>>(probed_ids + size_t(q0) * nprobe, probed_scores + size_t(q0) * nprobe, nqc, nprobe,
-                                            nlist, list_tile_start, list_rows, const_cast<uint32_t*>(ivf.list_mask),
-                                            const_cast<float*>(ivf.coarse), const_cast<int4*>(ivf.work), const_cast<int*>(ivf.n_work));
-    CRAG_CUDA_OK(cudaGetLastError());
-    // every CTA of the grid publishes a (possibly empty) partial list, so the merge always reads sp.grid parts
-    uint64_t* pool = nullptr;
-    if (sp.pool_bytes) {
-      pool = reinterpret_cast<uint64_t*>(ws + ip.pool_off);
-      CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, sp.pool_bytes, stream));
-    }
-    rc = launch_topk_scan<true>(tm_res, tm_q, 0, num_kb, nqc, k, sp.grid, nullptr, pool, 0u, 0, part_keys, part_minmax, ivf, stream);
-    if (rc != CRAG_OK) return rc;
-    rc = finalize_parts(workspace, sp.grid, nqc, k, 0, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
-                        out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, nullptr, sp, stream);
-    if (rc != CRAG_OK) return rc;
-    ivf_map_ids_kernel<<<(nqc * k + 255) / 256, 256, 0, stream>>>(out_ids + size_t(q0) * k, nqc * k, row_ids);
-    CRAG_CUDA_OK(cudaGetLastError());
-  }
-  return CRAG_OK;
+  return ivf_passes(res, q, IvfArgs{}, lists, k, k, nullptr, out_ids, out_scores, out_minmax, workspace, ip, sp,
+                    static_cast<cudaStream_t>(stream));
 }
 
-// ------------------------------------------------------------------ IVF over int8 residuals
-// Per 32-query pass: the IVF plan, the int8 scan of the probed tiles for n_cand candidates (S1 + coarse term), their
-// merge into the workspace, the exact bf16 rescore with the coarse term of each candidate's list (quant.cu), and the
-// map of stored positions to original ids.  The coarse table the rescore reads is the plan's, rebuilt every pass.
-namespace crag {
-namespace {
-struct IvfI8Plan {
-  IvfPlan ivf;
-  size_t cand_ids_off, cand_scores_off, total;
-};
-IvfI8Plan plan_ivf_i8(int nlist, int64_t total_tiles, int n_cand) {
-  IvfI8Plan p;
-  p.ivf = plan_ivf(plan_search(n_cand), nlist, total_tiles);
-  p.cand_ids_off = p.ivf.total;
-  p.cand_scores_off = p.cand_ids_off + ((size_t(kNQ) * n_cand * 8 + 255) & ~size_t(255));
-  p.total = p.cand_scores_off + ((size_t(kNQ) * n_cand * 4 + 255) & ~size_t(255));
-  return p;
-}
-}  // namespace
-}  // namespace crag
-
+// ------------------------------------------------------------------ IVF over int8 residuals (ivf_passes with a rescore)
 extern "C" size_t crag_ivf_i8_workspace_bytes(int nlist, int64_t total_tiles, int n_cand) {
   if (nlist < 1 || total_tiles < 0 || n_cand < 1 || n_cand > 128) return 0;
   return plan_ivf_i8(nlist, total_tiles, n_cand).total;
@@ -522,79 +582,40 @@ extern "C" int crag_ivf_search_i8(const void* residuals_i8, const float* row_sca
                                   const float* query_scales, const void* queries_bf16, int nq,
                                   const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand, int k,
                                   int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
-                                  size_t workspace_bytes, crag_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (nlist < 1 || nlist > (1 << 20) || nprobe < 1 || nprobe > nlist) return fail(CRAG_ERR_INVALID, "ivf_i8: need 1 <= nprobe <= nlist <= 2^20 (nprobe=%d nlist=%d)", nprobe, nlist);
+                                  size_t workspace_bytes, crag_stream_t stream) {
+  const Operand res{residuals_i8, n_rows_padded, dim8, row_stride_i8, kS8, "residuals_i8"}, q{queries_i8, nq, dim8, dim8, kS8, "queries_i8"};
+  IvfRescore rescore{{residuals_bf16, n_rows_padded, dim, row_stride, kBf16, "residuals_bf16"},
+                     {queries_bf16, nq, dim, dim, kBf16, "queries_bf16"}, nullptr, nullptr};
+  const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
+  int rc = check_ivf_args("ivf_i8", lists, n_rows_padded, out_ids, out_scores);
+  if (rc != CRAG_OK) return rc;
   if (nq < 1 || k < 1 || n_cand < k || n_cand > 128) return fail(CRAG_ERR_INVALID, "ivf_i8: need nq >= 1 and 1 <= k <= n_cand <= 128 (nq=%d k=%d n_cand=%d)", nq, k, n_cand);
-  if (dim < 64 || dim > 1024 || dim % 64 != 0) return fail(CRAG_ERR_INVALID, "ivf_i8: dim must be a multiple of 64 in [64, 1024] (dim=%d)", dim);
   if (dim8 != (dim + 127) / 128 * 128) return fail(CRAG_ERR_INVALID, "ivf_i8: dim8 must be dim rounded up to a multiple of 128 (dim=%d dim8=%d)", dim, dim8);
-  if (total_tiles < 1 || total_tiles * kTileRows != n_rows_padded || n_rows_padded >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "ivf_i8: need n_rows_padded (%lld) = total_tiles (%lld) * %d, non-empty and below 2^31", (long long)n_rows_padded, (long long)total_tiles, kTileRows);
-  if (row_stride_i8 < dim8 || row_stride_i8 % 16 != 0) return fail(CRAG_ERR_INVALID, "ivf_i8: row_stride_i8 must be >= dim8 and a multiple of 16");
-  if (row_stride < dim || row_stride % 8 != 0) return fail(CRAG_ERR_INVALID, "ivf_i8: row_stride must be >= dim and a multiple of 8");
-  if (!residuals_i8 || !row_scales || !residuals_bf16 || !list_tile_start || !list_rows || !row_ids || !queries_i8 ||
-      !query_scales || !queries_bf16 || !probed_ids || !probed_scores || !out_ids || !out_scores || !workspace) return fail(CRAG_ERR_INVALID, "ivf_i8: null pointer");
-  if ((reinterpret_cast<uintptr_t>(residuals_i8) | reinterpret_cast<uintptr_t>(queries_i8) | reinterpret_cast<uintptr_t>(residuals_bf16) |
-       reinterpret_cast<uintptr_t>(queries_bf16)) & 15) return fail(CRAG_ERR_INVALID, "ivf_i8: residuals and queries must be 16-byte aligned");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "ivf_i8: workspace must be 256-byte aligned");
   const IvfI8Plan plan = plan_ivf_i8(nlist, total_tiles, n_cand);
-  if (workspace_bytes < plan.total) return fail(CRAG_ERR_WORKSPACE, "ivf_i8: workspace %zu < %zu bytes", workspace_bytes, plan.total);
-  const void* rows_bf16 = nullptr;   // the bf16 residuals may be page-locked host memory: refused before any launch if pageable
-  int rc = device_readable(residuals_bf16, &rows_bf16, "ivf_i8");
+  rc = check_scan_args("ivf_i8", nq, n_cand, 128, res, q, workspace, workspace_bytes, plan.total);
+  if (rc == CRAG_OK) rc = check_operand("ivf_i8", rescore.rows);
+  if (rc == CRAG_OK) rc = check_operand("ivf_i8", rescore.queries);
   if (rc != CRAG_OK) return rc;
-  const SearchPlan sp = plan_search(n_cand);
+  if (!row_scales || !query_scales) return fail(CRAG_ERR_INVALID, "ivf_i8: null pointer");
+  // the bf16 residuals may be page-locked host memory: refused before any launch if pageable
+  rc = device_readable(residuals_bf16, &rescore.rows.ptr, "ivf_i8");
+  if (rc != CRAG_OK) return rc;
   uint8_t* ws = static_cast<uint8_t*>(workspace);
-  uint64_t* part_keys = reinterpret_cast<uint64_t*>(ws);
-  float* part_minmax = reinterpret_cast<float*>(ws + sp.keys_bytes);
-  int64_t* cand_ids = reinterpret_cast<int64_t*>(ws + plan.cand_ids_off);
-  float* cand_scores = reinterpret_cast<float*>(ws + plan.cand_scores_off);
-  I8IvfArgs args;
-  args.list_mask = reinterpret_cast<uint32_t*>(ws + plan.ivf.mask_off);
-  args.coarse = reinterpret_cast<float*>(ws + plan.ivf.coarse_off);
-  args.work = reinterpret_cast<int4*>(ws + plan.ivf.work_off);
-  args.n_work = reinterpret_cast<int*>(ws + plan.ivf.count_off);
-  args.row_scales = row_scales;
-  CUtensorMap tm_res;
-  rc = make_tmap_u8_2d(&tm_res, residuals_i8, uint64_t(n_rows_padded), uint64_t(dim8), uint64_t(row_stride_i8), kTileRows);
-  if (rc != CRAG_OK) return rc;
-  for (int q0 = 0; q0 < nq; q0 += kNQ) {
-    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
-    CUtensorMap tm_q;
-    rc = make_tmap_u8_2d(&tm_q, static_cast<const uint8_t*>(queries_i8) + size_t(q0) * dim8, uint64_t(nqc), uint64_t(dim8), uint64_t(dim8), kNQ);
-    if (rc != CRAG_OK) return rc;
-    ivf_plan_kernel<<<1, 1024, 0, stream>>>(probed_ids + size_t(q0) * nprobe, probed_scores + size_t(q0) * nprobe, nqc, nprobe,
-                                            nlist, list_tile_start, list_rows, const_cast<uint32_t*>(args.list_mask),
-                                            const_cast<float*>(args.coarse), const_cast<int4*>(args.work), const_cast<int*>(args.n_work));
-    CRAG_CUDA_OK(cudaGetLastError());
-    uint64_t* pool = nullptr;
-    if (sp.pool_bytes) {
-      pool = reinterpret_cast<uint64_t*>(ws + plan.ivf.pool_off);
-      CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, sp.pool_bytes, stream));
-    }
-    args.query_scales = query_scales + q0;
-    rc = launch_topk_scan<true>(tm_res, tm_q, int(n_rows_padded), dim8 / 128, nqc, n_cand, sp.grid, nullptr, pool, 0u, 0,
-                                part_keys, part_minmax, args, stream);
-    if (rc != CRAG_OK) return rc;
-    rc = finalize_parts(workspace, sp.grid, nqc, n_cand, 0, cand_ids, cand_scores,
-                        out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, nullptr, sp, stream);
-    if (rc != CRAG_OK) return rc;
-    rc = launch_ivf_rescore(rows_bf16, n_rows_padded, dim, row_stride, static_cast<const uint8_t*>(queries_bf16) + size_t(q0) * dim * 2,
-                            nqc, cand_ids, n_cand, k, list_tile_start, nlist, args.coarse, out_ids + size_t(q0) * k,
-                            out_scores + size_t(q0) * k, stream);
-    if (rc != CRAG_OK) return rc;
-    ivf_map_ids_kernel<<<(nqc * k + 255) / 256, 256, 0, stream>>>(out_ids + size_t(q0) * k, nqc * k, row_ids);
-    CRAG_CUDA_OK(cudaGetLastError());
-  }
-  return CRAG_OK;
+  rescore.cand_ids = reinterpret_cast<int64_t*>(ws + plan.cand_ids_off);
+  rescore.cand_scores = reinterpret_cast<float*>(ws + plan.cand_scores_off);
+  return ivf_passes(res, q, I8IvfArgs{{}, {row_scales, query_scales}}, lists, n_cand, k, &rescore, out_ids, out_scores, out_minmax, workspace, plan.ivf,
+                    plan_search(n_cand), static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int crag_search_scan(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,
                                 const void* queries, int nq, int k, void* workspace, size_t workspace_bytes,
                                 crag_stream_t stream) {
+  const Operand c{corpus, n_rows, dim, corpus_row_stride, kBf16, "corpus"}, q{queries, nq, dim, dim, kBf16, "queries"};
   const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1);
-  int rc = check_search_args(corpus, n_rows, dim, corpus_row_stride, queries, nq, k, workspace, workspace_bytes, plan);
+  int rc = check_scan_args("search", nq, k, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
   if (rc != CRAG_OK) return rc;
   if (nq > kNQ) return fail(CRAG_ERR_INVALID, "crag_search_scan handles one pass of at most %d queries (nq=%d)", kNQ, nq);
-  return scan_pass(corpus, n_rows, dim, corpus_row_stride, queries, 0, nq, k, nullptr, workspace, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
+  return scan_pass(c, q, k, nullptr, NoIvfArgs{}, workspace, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int crag_search_finalize(const void* workspace, size_t workspace_bytes, int64_t n_rows, int nq, int k,
@@ -604,28 +625,22 @@ extern "C" int crag_search_finalize(const void* workspace, size_t workspace_byte
   const SearchPlan plan = plan_search(k);
   if (!workspace || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "crag_search_finalize: null pointer");
   if (workspace_bytes < plan.keys_bytes + plan.minmax_bytes) return fail(CRAG_ERR_WORKSPACE, "crag_search_finalize: workspace too small");
-  return finalize_pass(workspace, n_rows, nq, k, row_offset, out_ids, out_scores, out_minmax, nullptr, plan, static_cast<cudaStream_t>(stream));
+  return finalize_parts(workspace, scan_grid(n_rows, plan), nq, k, row_offset, out_ids, out_scores, out_minmax, nullptr, plan,
+                        static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int crag_search_topk_after(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,
                                       int64_t row_offset, const void* queries, int nq, int k,
                                       const uint64_t* after_keys, int64_t* out_ids, float* out_scores,
                                       float* out_minmax, uint64_t* last_keys, void* workspace,
-                                      size_t workspace_bytes, crag_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+                                      size_t workspace_bytes, crag_stream_t stream) {
+  const Operand c{corpus, n_rows, dim, corpus_row_stride, kBf16, "corpus"}, q{queries, nq, dim, dim, kBf16, "queries"};
   const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1);
-  int rc = check_search_args(corpus, n_rows, dim, corpus_row_stride, queries, nq, k, workspace, workspace_bytes, plan);
+  int rc = check_scan_args("search", nq, k, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
   if (rc != CRAG_OK) return rc;
   if (!out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "search: null output pointer");
-  for (int q0 = 0; q0 < nq; q0 += kNQ) {
-    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
-    rc = scan_pass(corpus, n_rows, dim, corpus_row_stride, queries, q0, nqc, k, after_keys ? after_keys + q0 : nullptr, workspace, workspace_bytes, plan, stream);
-    if (rc != CRAG_OK) return rc;
-    rc = finalize_pass(workspace, n_rows, nqc, k, row_offset, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
-                       out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, last_keys ? last_keys + q0 : nullptr, plan, stream);
-    if (rc != CRAG_OK) return rc;
-  }
-  return CRAG_OK;
+  return topk_passes(c, q, k, row_offset, after_keys, NoIvfArgs{}, out_ids, out_scores, out_minmax, last_keys, workspace,
+                     workspace_bytes, plan, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int crag_search_topk(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,
@@ -640,27 +655,14 @@ extern "C" int crag_search_topk(const void* corpus, int64_t n_rows, int dim, int
 extern "C" int crag_search_topk_i8(const void* corpus_i8, const float* row_scales, int64_t n_rows, int dim8,
                                    int64_t row_stride, int64_t row_offset, const void* queries_i8,
                                    const float* query_scales, int nq, int k, int64_t* out_ids, float* out_scores,
-                                   float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+                                   float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream) {
+  const Operand c{corpus_i8, n_rows, dim8, row_stride, kS8, "corpus"}, q{queries_i8, nq, dim8, dim8, kS8, "queries"};
   const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1);
-  if (nq < 1 || k < 1 || k > 128) return fail(CRAG_ERR_INVALID, "search_i8: need nq >= 1 and 1 <= k <= 128 (nq=%d k=%d)", nq, k);
-  if (dim8 < 128 || dim8 > 1024 || dim8 % 128 != 0) return fail(CRAG_ERR_INVALID, "search_i8: dim8 must be a multiple of 128 in [128, 1024] (dim8=%d)", dim8);
-  if (n_rows < 0 || n_rows >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "search_i8: n_rows out of range (%lld)", (long long)n_rows);
-  if (row_stride < dim8 || row_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "search_i8: row_stride must be >= dim8 and a multiple of 16");
-  if (!queries_i8 || !query_scales || !workspace || !out_ids || !out_scores || (n_rows > 0 && (!corpus_i8 || !row_scales))) return fail(CRAG_ERR_INVALID, "search_i8: null pointer");
-  if ((reinterpret_cast<uintptr_t>(corpus_i8) | reinterpret_cast<uintptr_t>(queries_i8)) & 15) return fail(CRAG_ERR_INVALID, "search_i8: corpus/queries must be 16-byte aligned");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "search_i8: workspace must be 256-byte aligned");
-  if (workspace_bytes < plan.keys_bytes + plan.minmax_bytes) return fail(CRAG_ERR_WORKSPACE, "search_i8: workspace %zu < %zu bytes", workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
-  const I8Args i8{row_scales, query_scales};
-  for (int q0 = 0; q0 < nq; q0 += kNQ) {
-    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
-    int rc = scan_pass(corpus_i8, n_rows, dim8, row_stride, queries_i8, q0, nqc, k, nullptr, workspace, workspace_bytes, plan, stream, &i8);
-    if (rc != CRAG_OK) return rc;
-    rc = finalize_pass(workspace, n_rows, nqc, k, row_offset, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
-                       out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, nullptr, plan, stream);
-    if (rc != CRAG_OK) return rc;
-  }
-  return CRAG_OK;
+  int rc = check_scan_args("search_i8", nq, k, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
+  if (rc != CRAG_OK) return rc;
+  if (!query_scales || !out_ids || !out_scores || (n_rows > 0 && !row_scales)) return fail(CRAG_ERR_INVALID, "search_i8: null pointer");
+  return topk_passes(c, q, k, row_offset, nullptr, I8Args{row_scales, query_scales}, out_ids, out_scores, out_minmax,
+                     nullptr, workspace, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------ exact top-k for large k / many queries
@@ -681,9 +683,8 @@ extern "C" int crag_knn_topk(const void* corpus, int64_t n_rows, int dim, int64_
                              const void* queries, int nq, int k, int64_t* out_ids, float* out_scores, float* out_minmax,
                              void* workspace, size_t workspace_bytes, crag_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const SearchPlan no_scan_workspace{0, 0, 0, 0};
-  int rc = check_search_args(corpus, n_rows, dim, corpus_row_stride, queries, nq, k, workspace, workspace_bytes,
-                             no_scan_workspace, kKnnMaxK);
+  const Operand c{corpus, n_rows, dim, corpus_row_stride, kBf16, "corpus"}, q{queries, nq, dim, dim, kBf16, "queries"};
+  int rc = check_scan_args("search", nq, k, kKnnMaxK, c, q, workspace, workspace_bytes, 0);
   if (rc != CRAG_OK) return rc;
   if (!out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "knn: null output pointer");
   const int64_t ld = knn_ld(n_rows);
@@ -761,12 +762,13 @@ __global__ void minmax_reduce_kernel(const float* __restrict__ part_minmax, int 
   }
 }
 
-// Score-all passes (the scan with SCORES), one per block of 32 queries.  Block q0 stores its scores from row q0 of
+// Score-all passes (the scan with ScoreArgs), one per block of 32 queries.  Block q0 stores its scores from row q0 of
 // sa.out on, or, in assignment mode (sa.best_id set), updates every row's running argmax with ids counted from q0.
 // out_minmax (may be null) receives each query's (min, max).
-int score_passes(const void* corpus, int64_t n_rows, int dim, int64_t row_stride, const void* queries, int nq,
-                 ScoreArgs sa, float* out_minmax, void* workspace, const SearchPlan& plan, cudaStream_t stream) {
-  const int grid = scan_grid(n_rows, plan);
+int score_passes(const Operand& corpus, const Operand& queries, ScoreArgs sa, float* out_minmax, void* workspace,
+                 const SearchPlan& plan, cudaStream_t stream) {
+  const int nq = int(queries.rows);
+  const int grid = scan_grid(corpus.rows, plan);
   if (grid == 0) {
     if (out_minmax) {   // empty shard: (+inf, -inf), as crag_search_topk
       minmax_reduce_kernel<<<nq, 32, 0, stream>>>(nullptr, 0, nq, out_minmax);
@@ -776,17 +778,17 @@ int score_passes(const void* corpus, int64_t n_rows, int dim, int64_t row_stride
   }
   float* part_minmax = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + plan.keys_bytes);
   CUtensorMap tm_corpus;
-  int rc = make_tmap_bf16_2d(&tm_corpus, corpus, uint64_t(n_rows), uint64_t(dim), uint64_t(row_stride) * 2, kTileRows);
+  int rc = make_tmap(&tm_corpus, corpus, kTileRows);
   if (rc != CRAG_OK) return rc;
   for (int q0 = 0; q0 < nq; q0 += kNQ) {
     const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
     CUtensorMap tm_q;
-    rc = make_query_tmap(&tm_q, queries, q0, nqc, dim);
+    rc = make_tmap(&tm_q, queries.rows_from(q0, nqc), kNQ);
     if (rc != CRAG_OK) return rc;
     ScoreArgs pass = sa;
     if (sa.best_id) pass.base_id = q0;
     else pass.out = sa.out + int64_t(q0) * sa.ld;
-    rc = launch_scan<16, 16, 7, false, true>(tm_corpus, tm_q, int(n_rows), dim / kBlockK, nqc, 1, grid, nullptr, nullptr, 0u, 0, nullptr, part_minmax, pass, stream);
+    rc = launch_scan<16, 16, 7>(tm_corpus, tm_q, int(corpus.rows), corpus.num_kb(), nqc, 1, grid, nullptr, nullptr, 0u, 0, nullptr, part_minmax, pass, stream);
     if (rc != CRAG_OK) return rc;
     if (out_minmax) {
       minmax_reduce_kernel<<<nqc, 32, 0, stream>>>(part_minmax, grid, nqc, out_minmax + size_t(q0) * 2);
@@ -801,12 +803,13 @@ int score_passes(const void* corpus, int64_t n_rows, int dim, int64_t row_stride
 extern "C" int crag_search_scores(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,
                                   const void* queries, int nq, float* out_scores, int64_t out_ld, float* out_minmax,
                                   void* workspace, size_t workspace_bytes, crag_stream_t stream) {
+  const Operand c{corpus, n_rows, dim, corpus_row_stride, kBf16, "corpus"}, q{queries, nq, dim, dim, kBf16, "queries"};
   const SearchPlan plan = plan_search(1);
-  int rc = check_search_args(corpus, n_rows, dim, corpus_row_stride, queries, nq, 1, workspace, workspace_bytes, plan);
+  int rc = check_scan_args("search", nq, 1, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
   if (rc != CRAG_OK) return rc;
   if (!out_scores || out_ld < n_rows) return fail(CRAG_ERR_INVALID, "crag_search_scores: need out_scores and out_ld >= n_rows");
-  return score_passes(corpus, n_rows, dim, corpus_row_stride, queries, nq, ScoreArgs{out_scores, out_ld, nullptr, nullptr, 0}, out_minmax, workspace,
-                      plan, static_cast<cudaStream_t>(stream));
+  return score_passes(c, q, ScoreArgs{out_scores, out_ld, nullptr, nullptr, 0}, out_minmax, workspace, plan,
+                      static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------ fused finalize + exchange (row-sharded index)
@@ -844,11 +847,12 @@ extern "C" int crag_search_finalize_exchange(const void* workspace, size_t works
 extern "C" int crag_ivf_assign(const void* rows, int64_t n_rows, int dim, int64_t row_stride, const void* centroids,
                                int nlist, float* best_score, int32_t* best_id, void* workspace, size_t workspace_bytes,
                                crag_stream_t stream) {
+  const Operand c{rows, n_rows, dim, row_stride, kBf16, "rows"}, q{centroids, nlist, dim, dim, kBf16, "centroids"};
   const SearchPlan plan = plan_search(1);
-  int rc = check_search_args(rows, n_rows, dim, row_stride, centroids, nlist, 1, workspace, workspace_bytes, plan);
+  int rc = check_scan_args("search", nlist, 1, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
   if (rc != CRAG_OK) return rc;
   if (!best_score || !best_id) return fail(CRAG_ERR_INVALID, "crag_ivf_assign: null output pointer");
   // the pass over centroid block 0 initialises every row's running best (-inf, list 0); later passes update it
-  return score_passes(rows, n_rows, dim, row_stride, centroids, nlist, ScoreArgs{nullptr, 0, best_score, best_id, 0}, nullptr, workspace, plan,
+  return score_passes(c, q, ScoreArgs{nullptr, 0, best_score, best_id, 0}, nullptr, workspace, plan,
                       static_cast<cudaStream_t>(stream));
 }

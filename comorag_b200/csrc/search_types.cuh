@@ -3,6 +3,7 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+#include <type_traits>
 #include <cuda_runtime.h>
 
 #include "ivf_kernels.cuh"
@@ -37,7 +38,7 @@ constexpr int kAccStages = 4;
 //   work[i]   = (first stored row of the tile, valid rows in it, list id, 0), written by ivf_plan_kernel
 //   n_work    = number of work items (device scalar: the plan is built on the device, no host round trip)
 //   list_mask = per list, bit q set when query q probes it; coarse[list * 32 + q] = q . c_list from the coarse pass
-// The flat instantiations (IVF = false) take an empty struct instead and compile to the same SASS as before.
+// The flat top-k scan takes an empty struct instead.
 // r[q] for a runtime q without sending the score registers to local memory: a 5-level select tree on the bits of q
 __device__ __forceinline__ uint32_t pick32(const uint32_t (&r)[32], int q) {
   uint32_t a[16], b[8], c[4], d[2];
@@ -59,7 +60,7 @@ struct IvfArgs {
   const float* coarse;
 };
 struct NoIvfArgs {};
-// Score-all variant (SCORES = true): the full-array contracts of the reference -- get_fact_scores returns the score
+// Score-all variant (ScoreArgs): the full-array contracts of the reference -- get_fact_scores returns the score
 // of EVERY fact row (ComoRAG.py:937-948) and dense_passage_retrieval a permutation of ALL rows (:950-967, consumed
 // rank by rank by PPR at :1034-1042).  Same TMA -> wgmma -> score-tile stream; the select warps write the fp32 scores
 // (out[q * ld + row], one coalesced 128-byte store per warp and query) instead of running the selector.
@@ -73,6 +74,10 @@ struct ScoreArgs {
   int32_t* best_id;
   int32_t base_id;
 };
+// A scan variant is named by its argument struct; the select warps take it as the flags IVF / SCORES, which IvfParam
+// maps back to a bf16 variant's struct (tests/warp_emu/select_shell.h).
+template <class Args> constexpr bool kIvfScan = std::is_base_of<IvfArgs, Args>::value;
+template <class Args> constexpr bool kScoreScan = std::is_same<Args, ScoreArgs>::value;
 template <bool IVF, bool SCORES> struct IvfParam { using type = NoIvfArgs; };
 template <> struct IvfParam<true, false> { using type = IvfArgs; };
 template <> struct IvfParam<false, true> { using type = ScoreArgs; };

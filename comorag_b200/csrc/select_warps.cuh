@@ -181,12 +181,12 @@ struct SelectSmem {
 // The body of select warp `warp` (0-3): every score tile of this CTA, then the drain of the candidate buffers and this
 // CTA's lists and (min, max) in part_keys / part_minmax.  Each thread owns one row of a tile: it takes that row's kNQ
 // scores from tiles.next(tile, quad, lane, r), updates the per-query (min, max) and offers the scores that beat the
-// query's threshold to the candidate buffers.  IVF walks a work-list of probed tiles; SCORES stores every score
-// (or keeps each row's running argmax) instead of selecting.
-template <int KLIST, int CAP, bool IVF, bool SCORES, class Tiles>
+// query's threshold to the candidate buffers.  IVF walks the work-list of `args`, the scan's argument struct; SCORES
+// stores every score (or keeps each row's running argmax) in the outputs of `args` instead of selecting.
+template <int KLIST, int CAP, bool IVF, bool SCORES, class Tiles, class Args>
 __device__ __forceinline__ void select_warps(const SelectSmem<KLIST, CAP> s, Tiles& tiles, const TileOrder order, int num_tiles, int n_rows,
                                              int nq, int k, const uint64_t* after_keys, uint64_t* pool, uint64_t* part_keys,
-                                             float* part_minmax, const typename IvfParam<IVF, SCORES>::type& args, int warp, int lane) {
+                                             float* part_minmax, const Args& args, int warp, int lane) {
   constexpr int KPQ = KLIST + CAP;
   const int quad = warp;      // rows quad * 32 .. quad * 32 + 31 of every score tile
   const int ew = warp;        // select-warp index 0..3 (query ownership for flushes)

@@ -109,7 +109,50 @@ def assign_rows(x: torch.Tensor, centroids_bf16: torch.Tensor, block: int = 1 <<
     return out
 
 
-class IVFIndex:
+class _IVFSearch:
+    """The search plumbing IVFIndex and QuantizedIVF share; a subclass sets device, dim, nlist and centroids."""
+
+    def _search(self, queries_bf16: torch.Tensor, nprobe: int, k: int, stream: Optional[torch.cuda.Stream],
+                probed: Optional[Tuple[torch.Tensor, torch.Tensor]], ws_bytes: int, fine):
+        """search_device's common part: the nprobe and query checks, the coarse pass or the check of the caller's
+        `probed`, the outputs and the workspace.  fine(q, p_ids, p_scores, ids, scores, minmax, ws, st) runs the
+        native fine pass on stream st."""
+        if not 1 <= nprobe <= min(MAX_K, self.nlist):
+            raise ValueError(f"nprobe must be in [1, {min(MAX_K, self.nlist)}]")
+        if (queries_bf16.dtype != torch.bfloat16 or queries_bf16.dim() != 2 or queries_bf16.shape[1] != self.dim
+                or queries_bf16.device != self.device):
+            raise ValueError(f"queries must be bf16 [nq, {self.dim}] on {self.device}")
+        q = queries_bf16.contiguous()
+        nq, dev = q.shape[0], self.device
+        with torch.cuda.device(dev):
+            st = stream if stream is not None else torch.cuda.current_stream(dev)
+            with torch.cuda.stream(st):
+                if probed is None:
+                    p_ids, p_scores, _ = self.centroids.search_device(q, nprobe, stream=st)
+                else:
+                    p_ids, p_scores = (t.contiguous() for t in probed)
+                    if (p_ids.dtype != torch.int64 or p_scores.dtype != torch.float32 or
+                            tuple(p_ids.shape) != (nq, nprobe) or tuple(p_scores.shape) != (nq, nprobe) or
+                            p_ids.device != dev or p_scores.device != dev):
+                        raise ValueError(f"probed must be (int64 [nq, {nprobe}], fp32 [nq, {nprobe}]) on {dev}")
+                ids = torch.empty((nq, k), dtype=torch.int64, device=dev)
+                scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
+                minmax = torch.empty((nq, 2), dtype=torch.float32, device=dev)
+                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+                fine(q, p_ids, p_scores, ids, scores, minmax, ws, st)
+        return ids, scores, minmax, (p_ids, p_scores)
+
+    def search(self, queries, nprobe: int, k: int, *args, **kw) -> Tuple[np.ndarray, np.ndarray]:
+        """Host float [nq, dim] -> (ids int64 [nq, k], scores fp32 [nq, k]) as numpy; other arguments as search_device's."""
+        q = torch.as_tensor(queries)
+        if q.dim() == 1:
+            q = q[None, :]
+        q = q.to(self.device, non_blocking=True).to(torch.bfloat16)
+        ids, scores, _, _ = self.search_device(q, nprobe, k, *args, **kw)
+        return ids.cpu().numpy(), scores.cpu().numpy()
+
+
+class IVFIndex(_IVFSearch):
     def __init__(self, centroids_bf16: torch.Tensor, residuals: torch.Tensor, row_ids: torch.Tensor,
                  list_tile_start: torch.Tensor, list_rows: torch.Tensor, n_rows: int):
         """row_ids carry GLOBAL ids: a rank of a row-sharded index builds with row_offset = its first global row."""
@@ -160,43 +203,18 @@ class IVFIndex:
         (probed list ids int64 [nq, nprobe], their coarse scores fp32)).  1 <= k <= 128, 1 <= nprobe <= min(128, nlist)."""
         if not 1 <= k <= MAX_K:
             raise ValueError(f"k must be in [1, {MAX_K}]")
-        if not 1 <= nprobe <= min(MAX_K, self.nlist):
-            raise ValueError(f"nprobe must be in [1, {min(MAX_K, self.nlist)}]")
-        if queries_bf16.dtype != torch.bfloat16 or queries_bf16.dim() != 2 or queries_bf16.shape[1] != self.dim:
-            raise ValueError(f"queries must be bf16 [nq, {self.dim}]")
-        q = queries_bf16.contiguous()
-        nq, dev = q.shape[0], self.device
-        with torch.cuda.device(dev):
-            st = stream if stream is not None else torch.cuda.current_stream(dev)
-            with torch.cuda.stream(st):
-                if probed is None:
-                    p_ids, p_scores, _ = self.centroids.search_device(q, nprobe, stream=st)
-                else:
-                    p_ids, p_scores = (t.contiguous() for t in probed)
-                ids = torch.empty((nq, k), dtype=torch.int64, device=dev)
-                scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
-                minmax = torch.empty((nq, 2), dtype=torch.float32, device=dev)
-                ws_bytes = self._lib.crag_ivf_workspace_bytes(self.nlist, self.total_tiles, k)
-                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-                rc = self._lib.crag_ivf_search(
-                    self.residuals.data_ptr(), self.residuals.shape[0], self.dim, self.residuals.stride(0),
-                    self.list_tile_start.data_ptr(), self.list_rows.data_ptr(), self.nlist, self.total_tiles,
-                    self.row_ids.data_ptr(), q.data_ptr(), nq, p_ids.data_ptr(), p_scores.data_ptr(), nprobe, k,
-                    ids.data_ptr(), scores.data_ptr(), minmax.data_ptr(), ws.data_ptr(), ws_bytes, st.cuda_stream)
-                _native.check(rc, "crag_ivf_search")
-        return ids, scores, minmax, (p_ids, p_scores)
 
-    def search(self, queries, nprobe: int, k: int) -> Tuple[np.ndarray, np.ndarray]:
-        """Host float [nq, dim] -> (ids int64 [nq, k], scores fp32 [nq, k]) as numpy."""
-        q = torch.as_tensor(queries)
-        if q.dim() == 1:
-            q = q[None, :]
-        q = q.to(self.device, non_blocking=True).to(torch.bfloat16)
-        ids, scores, _, _ = self.search_device(q, nprobe, k)
-        return ids.cpu().numpy(), scores.cpu().numpy()
+        def fine(q, p_ids, p_scores, ids, scores, minmax, ws, st):
+            _native.check(self._lib.crag_ivf_search(
+                self.residuals.data_ptr(), self.residuals.shape[0], self.dim, self.residuals.stride(0),
+                self.list_tile_start.data_ptr(), self.list_rows.data_ptr(), self.nlist, self.total_tiles,
+                self.row_ids.data_ptr(), q.data_ptr(), q.shape[0], p_ids.data_ptr(), p_scores.data_ptr(), nprobe, k,
+                ids.data_ptr(), scores.data_ptr(), minmax.data_ptr(), ws.data_ptr(), ws.numel(), st.cuda_stream), "crag_ivf_search")
+        return self._search(queries_bf16, nprobe, k, stream, probed,
+                            self._lib.crag_ivf_workspace_bytes(self.nlist, self.total_tiles, k), fine)
 
 
-class QuantizedIVF:
+class QuantizedIVF(_IVFSearch):
     """Frozen int8 snapshot of an IVFIndex (crag_ivf_search_i8; DESIGN.md section 7).  Every stored residual row is
     quantised to int8 with one fp32 scale; a search scans the probed tiles' int8 residuals for `candidates` positions
     per query (S1 = int8 dot * scales + coarse term) and rescores those exactly from their bf16 residuals
@@ -254,48 +272,20 @@ class QuantizedIVF:
             candidates = min(MAX_K, 4 * k)
         if not 1 <= k <= candidates <= MAX_K:
             raise ValueError(f"need 1 <= k <= candidates <= {MAX_K} (k={k}, candidates={candidates})")
-        if not 1 <= nprobe <= min(MAX_K, self.nlist):
-            raise ValueError(f"nprobe must be in [1, {min(MAX_K, self.nlist)}]")
-        if (queries_bf16.dtype != torch.bfloat16 or queries_bf16.dim() != 2 or queries_bf16.shape[1] != self.dim
-                or queries_bf16.device != self.device):
-            raise ValueError(f"queries must be bf16 [nq, {self.dim}] on {self.device}")
         from .quantized import quantize_rows
-        q = queries_bf16.contiguous()
-        nq, dev = q.shape[0], self.device
-        with torch.cuda.device(dev):
-            st = stream if stream is not None else torch.cuda.current_stream(dev)
-            with torch.cuda.stream(st):
-                if probed is None:
-                    p_ids, p_scores, _ = self.centroids.search_device(q, nprobe, stream=st)
-                else:
-                    p_ids, p_scores = (t.contiguous() for t in probed)
-                    if (p_ids.dtype != torch.int64 or p_scores.dtype != torch.float32 or
-                            tuple(p_ids.shape) != (nq, nprobe) or tuple(p_scores.shape) != (nq, nprobe)):
-                        raise ValueError(f"probed must be (int64 [nq, {nprobe}], fp32 [nq, {nprobe}])")
-                q8, qs = quantize_rows(q, self.dim8, st)
-                ids = torch.empty((nq, k), dtype=torch.int64, device=dev)
-                scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
-                minmax = torch.empty((nq, 2), dtype=torch.float32, device=dev)
-                ws_bytes = self._lib.crag_ivf_i8_workspace_bytes(self.nlist, self.total_tiles, candidates)
-                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-                rc = self._lib.crag_ivf_search_i8(
-                    self._i8.data_ptr(), self._scales.data_ptr(), self.dim8, self._i8.stride(0),
-                    self._rows.data_ptr(), self.dim, self._rows.stride(0), self._rows.shape[0],
-                    self.list_tile_start.data_ptr(), self.list_rows.data_ptr(), self.nlist, self.total_tiles,
-                    self.row_ids.data_ptr(), q8.data_ptr(), qs.data_ptr(), q.data_ptr(), nq,
-                    p_ids.data_ptr(), p_scores.data_ptr(), nprobe, candidates, k,
-                    ids.data_ptr(), scores.data_ptr(), minmax.data_ptr(), ws.data_ptr(), ws_bytes, st.cuda_stream)
-                _native.check(rc, "crag_ivf_search_i8")
-        return ids, scores, minmax, (p_ids, p_scores)
 
-    def search(self, queries, nprobe: int, k: int, candidates: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray]:
-        """Host float [nq, dim] -> (ids int64 [nq, k], scores fp32 [nq, k]) as numpy."""
-        q = torch.as_tensor(queries)
-        if q.dim() == 1:
-            q = q[None, :]
-        q = q.to(self.device, non_blocking=True).to(torch.bfloat16)
-        ids, scores, _, _ = self.search_device(q, nprobe, k, candidates)
-        return ids.cpu().numpy(), scores.cpu().numpy()
+        def fine(q, p_ids, p_scores, ids, scores, minmax, ws, st):
+            q8, qs = quantize_rows(q, self.dim8, st)
+            _native.check(self._lib.crag_ivf_search_i8(
+                self._i8.data_ptr(), self._scales.data_ptr(), self.dim8, self._i8.stride(0),
+                self._rows.data_ptr(), self.dim, self._rows.stride(0), self._rows.shape[0],
+                self.list_tile_start.data_ptr(), self.list_rows.data_ptr(), self.nlist, self.total_tiles,
+                self.row_ids.data_ptr(), q8.data_ptr(), qs.data_ptr(), q.data_ptr(), q.shape[0],
+                p_ids.data_ptr(), p_scores.data_ptr(), nprobe, candidates, k,
+                ids.data_ptr(), scores.data_ptr(), minmax.data_ptr(), ws.data_ptr(), ws.numel(), st.cuda_stream),
+                "crag_ivf_search_i8")
+        return self._search(queries_bf16, nprobe, k, stream, probed,
+                            self._lib.crag_ivf_i8_workspace_bytes(self.nlist, self.total_tiles, candidates), fine)
 
 
 class ShardedIVF:

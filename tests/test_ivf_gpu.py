@@ -84,4 +84,10 @@ def test_ivf_argument_errors(dev):
     with pytest.raises(ValueError):
         idx.search_device(qb.float(), 2, 10)
     with pytest.raises(ValueError):
+        idx.search_device(qb.cpu(), 2, 10)           # queries on the host
+    p_ids, p_sc, _ = idx.centroids.search_device(qb, 2)
+    for probed in [(p_ids[:, :1], p_sc[:, :1]), (p_ids[:1], p_sc[:1]), (p_ids.to(torch.int32), p_sc)]:
+        with pytest.raises(ValueError):               # mis-shaped or int32 probed lists
+            idx.search_device(qb, 2, 10, probed=probed)
+    with pytest.raises(ValueError):
         IVFIndex.build(torch.from_numpy(x), 8)       # host tensor: no CPU fallback
