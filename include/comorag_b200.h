@@ -290,11 +290,16 @@ CRAG_API int crag_gemm_bf16(const void* a, int64_t lda, const void* w, int64_t l
  * padded with zero rows to whole 128-row tiles; list l owns tiles [list_tile_start[l], list_tile_start[l+1]) and
  * its first list_rows[l] rows are real; row_ids[stored row] = the row's original id (padding: -1).
  * The caller runs the coarse pass itself (crag_search_topk over the bf16 centroid table with k = nprobe) and
- * passes its output: probed_ids int64 [nq, nprobe] (-1 = absent), probed_scores fp32 [nq, nprobe] = q . c_list.
+ * passes its output: probed_ids int64 [nq, nprobe], probed_scores fp32 [nq, nprobe] = q . c_list.  A probed id
+ * of -1 or >= nlist is absent; a list probed twice by one query counts once (give both entries the same score:
+ * which one the plan keeps is unspecified).
  * Per block of 32 queries: a plan kernel marks which queries probe which list and compacts the probed lists'
  * tiles into a work-list; the scan kernel (the flat kernel's TMA/wgmma/selector pipeline walking that work-list)
- * scores  q . c_list + q . residual  for the probing queries only; the per-CTA lists are merged and stored-row ids
- * mapped to original ids.  Outputs as crag_search_topk (min/max range over the probed rows).
+ * scores  fp32(q . residual + q . c_list)  for the probing queries only; the per-CTA lists are merged and
+ * stored-row positions mapped to original ids.  Ranking: score descending, then STORED POSITION ascending (list
+ * id, then original id inside the list), so an exact tie between two lists goes to the smaller list id.  Outputs
+ * as crag_search_topk: -1 / -inf past the probed rows; out_minmax (may be NULL) is (min, max) over the probed
+ * real rows, (+inf, -inf) when there are none.
  * workspace >= crag_ivf_workspace_bytes(nlist, total_tiles, k), 256-byte aligned. */
 CRAG_API size_t crag_ivf_workspace_bytes(int nlist, int64_t total_tiles, int k);
 CRAG_API int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int dim, int64_t row_stride,

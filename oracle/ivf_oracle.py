@@ -14,8 +14,10 @@ is tested against a fixed semantic:
   search  for a query q (rounded to bf16, like the flat path): the `nprobe` lists of largest q.c_l (centroids
           rounded to bf16; ties: smaller list id) are probed; a row's score is  q.c_l + q.r  -- the coarse term is
           shared by the whole list and the fine term runs over the bf16 residuals, which is why the residual form
-          is more accurate than scoring bf16(x) directly (|r| << |x|); the answer is the k best (score descending,
-          original id ascending) among the probed lists only.
+          is more accurate than scoring bf16(x) directly (|r| << |x|); the answer is the k best among the probed
+          lists only, ranked by score descending, then by STORED POSITION ascending -- list id first, then original
+          id inside the list (the kernel keys on the position, a 32-bit word, and maps positions to 64-bit ids
+          afterwards).  So an exact tie between rows of two lists goes to the row of the smaller list id.
 
 `nprobe == nlist` degenerates to exact search over the reconstructed rows c_l + r.
 """
@@ -99,9 +101,11 @@ def probe_lists(lists: IVFLists, queries: np.ndarray, nprobe: int) -> Tuple[np.n
 
 def search(lists: IVFLists, queries: np.ndarray, nprobe: int, k: int, probed=None):
     """-> (ids int64 [nq, k], scores float64 [nq, k], gaps float64 [nq, k]); id -1 / score -inf where the probed
-    lists hold fewer than k rows.  gaps as in search_oracle.topk_exact (near ties are compared as sets).
-    `probed = (list ids [nq, nprobe], coarse scores)` replaces the coarse pass (ids < 0 are skipped): the fine
-    pass can then be checked on exactly the lists, and with exactly the fp32 coarse terms, the engine used."""
+    lists hold fewer than k rows.  gaps as in search_oracle.topk_exact (near ties are compared as sets).  Exact ties
+    go to the smaller stored position (list id, then original id).
+    `probed = (list ids [nq, nprobe], coarse scores)` replaces the coarse pass: the fine pass can then be checked on
+    exactly the lists, and with exactly the fp32 coarse terms, the engine used.  A list id < 0 or >= nlist is
+    absent, and a list probed twice counts once (with its first coarse score)."""
     q = bf16_round(queries).astype(np.float64)
     nq = q.shape[0]
     probed, coarse = probe_lists(lists, queries, min(nprobe, lists.nlist)) if probed is None else probed
@@ -109,19 +113,23 @@ def search(lists: IVFLists, queries: np.ndarray, nprobe: int, k: int, probed=Non
     out_s = np.full((nq, k), -np.inf)
     gaps = np.full((nq, k), np.inf)
     for i in range(nq):
-        cand_i: List[np.ndarray] = []
+        cand_p: List[np.ndarray] = []
         cand_s: List[np.ndarray] = []
+        seen = set()
         for l, cs in zip(probed[i], coarse[i]):
-            if l < 0:
+            l = int(l)
+            if l < 0 or l >= lists.nlist or l in seen:
                 continue
+            seen.add(l)
             a, b = lists.offsets[l], lists.offsets[l + 1]
             if b > a:
-                cand_i.append(lists.ids[a:b])
+                cand_p.append(np.arange(a, b))                     # stored positions: list order, then id
                 cand_s.append(np.float32(cs).astype(np.float64) + lists.residuals[a:b].astype(np.float64) @ q[i])
-        if not cand_i:
+        if not cand_p:
             continue
-        ci, cs_ = np.concatenate(cand_i), np.concatenate(cand_s)
-        order = np.lexsort((ci, -cs_))[:k + 1]
+        cp, cs_ = np.concatenate(cand_p), np.concatenate(cand_s)
+        order = np.lexsort((cp, -cs_))[:k + 1]
+        ci = lists.ids[cp]
         m = min(k, order.size)
         out_i[i, :m], out_s[i, :m] = ci[order[:m]], cs_[order[:m]]
         d = cs_[order[:-1]] - cs_[order[1:]]
