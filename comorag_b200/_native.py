@@ -94,6 +94,10 @@ SIGNATURES = {
                                      C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "crag_gmm_sweep_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
+    "crag_gmm_sweep": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 _lib = None

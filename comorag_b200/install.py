@@ -20,14 +20,16 @@ from typing import Dict
 
 
 def install(package: str = "src.comorag", rerank: bool = False, summaries: bool = True, search: bool = True,
-            knn: bool = True, encoder: bool = True, graph: bool = False) -> Dict[str, int]:
+            knn: bool = True, encoder: bool = True, graph: bool = False, cluster: bool = False) -> Dict[str, int]:
     """Returns {name: number of module attributes (or class methods) rebound}.  `rerank=True` also swaps the LLM
     filter for the dense reranker (new arithmetic, off by default so answers stay reference-identical); `search`
     rebinds the four ComoRAG retrieval methods, `knn` the synonymy-edge retrieve_knn; `encoder=False` keeps the
     reference's own embedding model class (HF, fp32) and swaps only the store / search half -- the parity tests use
     that to compare rankings without the bf16 encoder's error in the way.  `graph=True` also rebinds
     graph_search_with_fact_entities and run_ppr (comorag_methods.GRAPH_METHODS: PPR on the device, crag_ppr); it
-    needs a real igraph.Graph (get_edgelist, es["weight"]) and is off by default."""
+    needs a real igraph.Graph (get_edgelist, es["weight"]) and is off by default.  `cluster=True` rebinds
+    ChunkSoftClustering.perform_clustering (comorag_b200.cluster: the GMM sweeps on the device, crag_gmm_sweep; off
+    by default); the original stays reachable in the class's _comorag_b200_originals."""
     from . import embedding_model as em
     from . import embedding_store as es
     from . import rerank as rr
@@ -70,7 +72,25 @@ def install(package: str = "src.comorag", rerank: bool = False, summaries: bool 
                 originals[name] = cls.__dict__[name]
             setattr(cls, name, fn)
             counts["ComoRAG." + name] = 1
+    if cluster:
+        from . import cluster as cl
+        cls = importlib.import_module(package + ".utils.cluster_utils").ChunkSoftClustering
+        originals = cls.__dict__.get("_comorag_b200_originals")
+        if originals is None:
+            originals = {}
+            cls._comorag_b200_originals = originals
+        originals.setdefault("perform_clustering", cls.__dict__["perform_clustering"])
+        cls.perform_clustering = cl.perform_clustering
+        counts["ChunkSoftClustering.perform_clustering"] = 1
     return counts
+
+
+def uninstall_cluster(package: str = "src.comorag") -> None:
+    """Put the reference's own ChunkSoftClustering.perform_clustering back."""
+    mod = sys.modules.get(package + ".utils.cluster_utils")
+    originals = mod.ChunkSoftClustering.__dict__.get("_comorag_b200_originals") if mod is not None else None
+    if originals and "perform_clustering" in originals:
+        mod.ChunkSoftClustering.perform_clustering = originals["perform_clustering"]
 
 
 def uninstall_search(package: str = "src.comorag") -> None:

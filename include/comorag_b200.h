@@ -420,6 +420,36 @@ CRAG_API int crag_encoder_classify(const crag_encoder* model, const crag_classif
                                    int max_seqlen, float* logits, void* workspace, size_t workspace_bytes,
                                    crag_stream_t stream);
 
+/* The BIC sweep of ComoRAG's soft clustering (ChunkSoftClustering._get_optimal_clusters, cluster_utils.py:175-189,
+ * and the refit + predict_proba of the winner, :252-260): for m = 1..M (M = max_components), scikit-learn's
+ *     GaussianMixture(n_components=m, covariance_type="full", random_state=RandomState(224)).fit(x)
+ * restated in float64 -- k-means++ seeding and Lloyd (KMeans(n_clusters=m, n_init=1)), then EM from the one-hot
+ * k-means labels (reg_covar 1e-6, tol 1e-3, at most 100 iterations) -- and BIC_m on its final parameters.
+ * DESIGN.md section 2b.  The random draws of the seeding do not depend on the data; the caller makes them with
+ * numpy's RandomState(224), a fresh one per model, in scikit-learn's order:
+ *     first_centre[m - 1] = rs.choice(n, p=ones(n) / n)
+ *     seed_draws: model m's (m - 1) x (2 + int(log m)) values rs.uniform(size=2 + int(log m)), models in order
+ * All M models advance together; a model that has converged is frozen by a flag on the device.  No floating-point
+ * atomics: the same inputs give bit-identical outputs on every run and stream.
+ *   x              device fp64 [n][d], row-major; 2 <= n <= 2^31, 1 <= d <= 16, 1 <= M <= min(64, n - 1)
+ *   first_centre   device int64 [M];  seed_draws device fp64 [sum_m (m - 1)(2 + int(log m))] (NULL when M = 1)
+ *   out_bic        device fp64 [M];   out_iters, out_converged device int32 [M]: EM iterations and converged flag
+ *                  (1 when |change of the lower bound| < 1e-3, 0 after 100 iterations, -1 if a covariance was not
+ *                  positive definite)
+ *   out_best       device int32 [1]: the number of components with the smallest BIC (the first on a tie)
+ *   out_weights    device fp64 [M], out_means device fp64 [M][d]: the winner's first out_best entries
+ *   out_memberships device fp64 [n][out_best] (room for n * M): predict_proba of the winner
+ *   out_seeds      device int32 [M(M+1)/2] or NULL: model m's k-means++ rows at [m(m-1)/2, m(m+1)/2)
+ *   out_labels     device int32 [M][n] or NULL: model m's final k-means labels in row m - 1
+ *   workspace >= crag_gmm_sweep_workspace_bytes(n, d, M) bytes (0 for arguments out of range), 256-B aligned.
+ * Enqueues 2 * 300 + 2 * 100 + 10 kernels. */
+CRAG_API size_t crag_gmm_sweep_workspace_bytes(int64_t n, int d, int max_components);
+CRAG_API int crag_gmm_sweep(const double* x, int64_t n, int d, int max_components, const int64_t* first_centre,
+                            const double* seed_draws, double* out_bic, int32_t* out_iters, int32_t* out_converged,
+                            int32_t* out_best, double* out_weights, double* out_means, double* out_memberships,
+                            int32_t* out_seeds, int32_t* out_labels, void* workspace, size_t workspace_bytes,
+                            crag_stream_t stream);
+
 /* K3 on its own: masked mean pool + optional L2 normalise of a packed
  * last_hidden_state (bf16 [total_tokens, hidden_size]); mean_pooling
  * (BGEEmbedding.py:15-28) + F.normalize (:127). */
