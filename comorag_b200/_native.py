@@ -98,6 +98,16 @@ SIGNATURES = {
     "crag_gmm_sweep": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "crag_umap_fuzzy_graph_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "crag_umap_fuzzy_graph": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "crag_umap_spectral_init_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "crag_umap_spectral_init": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_uint64,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "crag_umap_optimize_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "crag_umap_optimize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_float,
+                                     C.c_float, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 _lib = None

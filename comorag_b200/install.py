@@ -20,7 +20,8 @@ from typing import Dict
 
 
 def install(package: str = "src.comorag", rerank: bool = False, summaries: bool = True, search: bool = True,
-            knn: bool = True, encoder: bool = True, graph: bool = False, cluster: bool = False) -> Dict[str, int]:
+            knn: bool = True, encoder: bool = True, graph: bool = False, cluster: bool = False,
+            umap: bool = False) -> Dict[str, int]:
     """Returns {name: number of module attributes (or class methods) rebound}.  `rerank=True` also swaps the LLM
     filter for the dense reranker (new arithmetic, off by default so answers stay reference-identical); `search`
     rebinds the four ComoRAG retrieval methods, `knn` the synonymy-edge retrieve_knn; `encoder=False` keeps the
@@ -29,7 +30,9 @@ def install(package: str = "src.comorag", rerank: bool = False, summaries: bool 
     graph_search_with_fact_entities and run_ppr (comorag_methods.GRAPH_METHODS: PPR on the device, crag_ppr); it
     needs a real igraph.Graph (get_edgelist, es["weight"]) and is off by default.  `cluster=True` rebinds
     ChunkSoftClustering.perform_clustering (comorag_b200.cluster: the GMM sweeps on the device, crag_gmm_sweep; off
-    by default); the original stays reachable in the class's _comorag_b200_originals."""
+    by default); the original stays reachable in the class's _comorag_b200_originals.  `umap=True` rebinds
+    ChunkSoftClustering._reduce_dimensions (comorag_b200.umap_layout: UMAP on the device, crag_umap_*; off by
+    default), with or without `cluster`."""
     from . import embedding_model as em
     from . import embedding_store as es
     from . import rerank as rr
@@ -82,15 +85,26 @@ def install(package: str = "src.comorag", rerank: bool = False, summaries: bool 
         originals.setdefault("perform_clustering", cls.__dict__["perform_clustering"])
         cls.perform_clustering = cl.perform_clustering
         counts["ChunkSoftClustering.perform_clustering"] = 1
+    if umap:
+        from . import umap_layout as ul
+        cls = importlib.import_module(package + ".utils.cluster_utils").ChunkSoftClustering
+        originals = cls.__dict__.get("_comorag_b200_originals")
+        if originals is None:
+            originals = {}
+            cls._comorag_b200_originals = originals
+        originals.setdefault("_reduce_dimensions", cls.__dict__["_reduce_dimensions"])
+        cls._reduce_dimensions = ul.reduce_dimensions
+        counts["ChunkSoftClustering._reduce_dimensions"] = 1
     return counts
 
 
 def uninstall_cluster(package: str = "src.comorag") -> None:
-    """Put the reference's own ChunkSoftClustering.perform_clustering back."""
+    """Put the reference's own ChunkSoftClustering.perform_clustering (and _reduce_dimensions, if rebound) back."""
     mod = sys.modules.get(package + ".utils.cluster_utils")
     originals = mod.ChunkSoftClustering.__dict__.get("_comorag_b200_originals") if mod is not None else None
-    if originals and "perform_clustering" in originals:
-        mod.ChunkSoftClustering.perform_clustering = originals["perform_clustering"]
+    for name in ("perform_clustering", "_reduce_dimensions"):
+        if originals and name in originals:
+            setattr(mod.ChunkSoftClustering, name, originals[name])
 
 
 def uninstall_search(package: str = "src.comorag") -> None:

@@ -450,6 +450,54 @@ CRAG_API int crag_gmm_sweep(const double* x, int64_t n, int d, int max_component
                             int32_t* out_seeds, int32_t* out_labels, void* workspace, size_t workspace_bytes,
                             crag_stream_t stream);
 
+/* UMAP for ChunkSoftClustering._reduce_dimensions (cluster_utils.py:191-211), in three stages that each run alone:
+ * umap-learn 0.5's UMAP(n_neighbors, n_components, metric="cosine") with its default parameters, with a subspace-
+ * iteration spectral start and snapshot layout epochs (DESIGN.md section 2c).  Raw device pointers; nothing allocates
+ * or waits for the host; no floating-point atomics: the same inputs give bit-identical outputs on every run and stream.
+ *
+ * crag_umap_fuzzy_graph: crag_knn_topk's self-join (knn_ids int64 / knn_scores fp32 [n][k], the rows L2-normalised)
+ * -> each row's list i, then its k - 1 best other rows (i's own entry removed where the search returned it, else the
+ * last entry dropped), out_nbr int32 [n][k] and out_dist fp32 [n][k] = max(0, 1 - score) (0 for i itself);
+ * out_rho / out_sigma fp32 [n] (smooth kNN: the first nonzero distance; 64 bisection steps toward log2(k), floored at
+ * 1e-3 x the row's mean distance, or the mean of all distances where rho = 0); out_memb fp32 [n][k], the directed
+ * memberships (0 on i itself).  2 <= n <= 2^30, 1 <= k <= min(256, n).
+ *   workspace >= crag_umap_fuzzy_graph_workspace_bytes(n, k) bytes (0 for arguments out of range), 256-B aligned. */
+CRAG_API size_t crag_umap_fuzzy_graph_workspace_bytes(int64_t n, int k);
+CRAG_API int crag_umap_fuzzy_graph(const int64_t* knn_ids, const float* knn_scores, int64_t n, int k, int32_t* out_nbr,
+                                   float* out_dist, float* out_rho, float* out_sigma, float* out_memb, void* workspace,
+                                   size_t workspace_bytes, crag_stream_t stream);
+
+/* crag_umap_spectral_init: the start layout from the symmetric fuzzy graph G (CSR: indptr int64 [n + 1], indices int32
+ * ascending within a row, weights fp32).  Block subspace iteration with p = min(max(16, d + 1), n) columns on
+ * S' = (I + D^-1/2 G D^-1/2) / 2 for `iters` steps (CholQR in fp64 after each), then Rayleigh-Ritz (cyclic Jacobi in
+ * fp64); Ritz vectors 2..d+1 by descending eigenvalue, each signed so its largest-magnitude entry is positive, then
+ * umap-learn's post-processing: x 10 / max|Y|, + 1e-4 N(0, 1) noise from the counter hash of `seed`, per-column
+ * min-max rescale to [0, 10].  n <= 16 runs no iteration (p = n).  1 <= d <= min(16, n - 1); iters >= 1 for n > 16.
+ *   out_y           device fp32 [n][d]
+ *   out_vectors     device fp64 [n][d] or NULL: the signed Ritz vectors before the post-processing
+ *   out_eigenvalues device fp64 [p] or NULL: the Ritz values, descending
+ *   workspace >= crag_umap_spectral_init_workspace_bytes(n, d) bytes, 256-B aligned. */
+CRAG_API size_t crag_umap_spectral_init_workspace_bytes(int64_t n, int d);
+CRAG_API int crag_umap_spectral_init(const int64_t* indptr, const int32_t* indices, const float* weights, int64_t n,
+                                     int d, int iters, uint64_t seed, float* out_y, double* out_vectors,
+                                     double* out_eigenvalues, void* workspace, size_t workspace_bytes,
+                                     crag_stream_t stream);
+
+/* crag_umap_optimize: layout epochs [epoch_begin, epoch_end) of n_epochs from y0 (device fp32 [n][d], may equal out_y)
+ * into out_y.  Epoch e (alpha = 1 - max(e - 1, 0) / n_epochs): every vertex i moves from its own current position
+ * while every other vertex is read from the previous epoch's snapshot; for each edge p of row i with
+ * next_sample[p] <= e, the attraction twice (edge (i, j), then (j, i) with i as the moved tail), then
+ * floor((e - next_neg[p]) / (epochs_per_sample[p] / 5)) negative samples whose targets are the counter hash of
+ * (seed, e, p, sample) mod n (a sample that hits i, or a coincident point, contributes 0); gradients clipped to +-4.
+ * next_sample / next_neg (device fp64 [nnz], in/out) are the schedule counters: epochs_per_sample and
+ * epochs_per_sample / 5 before epoch 0.  1 <= d <= 16.
+ *   workspace >= crag_umap_optimize_workspace_bytes(n, d) bytes (the second buffer), 256-B aligned. */
+CRAG_API size_t crag_umap_optimize_workspace_bytes(int64_t n, int d);
+CRAG_API int crag_umap_optimize(const int64_t* indptr, const int32_t* indices, const double* epochs_per_sample,
+                                int64_t n, int64_t nnz, int d, float a, float b, int n_epochs, int epoch_begin,
+                                int epoch_end, uint64_t seed, double* next_sample, double* next_neg, const float* y0,
+                                float* out_y, void* workspace, size_t workspace_bytes, crag_stream_t stream);
+
 /* K3 on its own: masked mean pool + optional L2 normalise of a packed
  * last_hidden_state (bf16 [total_tokens, hidden_size]); mean_pooling
  * (BGEEmbedding.py:15-28) + F.normalize (:127). */
