@@ -50,6 +50,16 @@ int make_tmap_2d(CUtensorMap* out, CUtensorMapDataType type, const void* base, u
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return fail(CRAG_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (driver too old?)");
   if (rows == 0 || cols == 0) return fail(CRAG_ERR_INVALID, "tensor map over an empty tensor");
+  // The encode needs a current context.  A host thread whose first CUDA call this is (its tensors all came from the
+  // allocator's cache) has none yet, and the encode fails with CUDA_ERROR_INVALID_CONTEXT: bind the primary context
+  // of the thread's current device first, once per thread.
+  thread_local bool bound = false;
+  if (!bound) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaSetDevice(dev) != cudaSuccess)
+      return fail(CRAG_ERR_CUDA, "no CUDA context for the tensor map: %s", cudaGetErrorString(cudaGetLastError()));
+    bound = true;
+  }
   const cuuint64_t gdim[2] = {cols, rows};
   const cuuint64_t gstride[1] = {row_stride_bytes};
   const cuuint32_t box[2] = {box_cols, box_rows};

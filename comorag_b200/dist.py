@@ -50,17 +50,38 @@ def unpack_partials(buf: torch.Tensor, world: int, nq: int, k: int) -> Tuple[tor
     return ids, scores, minmax
 
 
+def _orderable(x: torch.Tensor) -> torch.Tensor:
+    """The kernels' orderable_f32 of fp32 values, as int64 in [0, 2^32): unsigned order = score order, +0 above -0."""
+    u = x.contiguous().to(torch.float32).view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+    return torch.where(u >= (1 << 31), (~u) & 0xFFFFFFFF, u | (1 << 31))
+
+
 def merge_partials_reference(ids: torch.Tensor, scores: torch.Tensor, minmax: torch.Tensor, k: int):
-    """Plain-torch statement of the merge rule (score desc, then (rank, position) asc) used by the CPU/gloo
-    tests of the exchange step; the product path runs crag_merge_topk on the device."""
+    """Plain-torch statement of the merge rule of crag_merge_topk (used by the CPU/gloo tests of the exchange step;
+    the product path runs the kernel on the device).  Candidate j of rank p sits at position c = p * k + j and ranks
+    by the kernels' key orderable(score) << 32 | (0xFFFFFFFF - c): score descending with +0 above -0, then rank, then
+    position.  A candidate is absent iff its id < 0; a valid id with score -inf is kept.  -1 / -inf past the valid
+    candidates; (min, max) over the ranks in the same score order, (+inf, -inf) from no rank."""
     world, nq, kk = scores.shape
-    s = scores.permute(1, 0, 2).reshape(nq, world * kk).clone()
-    i = ids.permute(1, 0, 2).reshape(nq, world * kk)
-    s[i < 0] = float("-inf")
-    order = torch.argsort(s, dim=1, descending=True, stable=True)[:, :k]
-    out_s, out_i = torch.gather(s, 1, order), torch.gather(i, 1, order)
-    out_i = torch.where(torch.isinf(out_s) & (out_s < 0), torch.full_like(out_i, -1), out_i)
-    mm = torch.stack([minmax[..., 0].min(dim=0).values, minmax[..., 1].max(dim=0).values], dim=1)
+    n = world * kk
+    s = scores.permute(1, 0, 2).reshape(nq, n).to(torch.float32)
+    i = ids.permute(1, 0, 2).reshape(nq, n).to(torch.int64)
+    c = torch.arange(n, device=s.device, dtype=torch.int64)
+    key = (_orderable(s) - (1 << 31)) * (1 << 32) + (0xFFFFFFFF - c)      # the unsigned key, shifted into int64
+    key = torch.where(i >= 0, key, torch.full_like(key, -(1 << 63)))
+    top, col = torch.sort(key, dim=1, descending=True)
+    top, col = top[:, :k], col[:, :k]
+    present = top != -(1 << 63)
+    out_i = torch.full((nq, k), -1, dtype=torch.int64, device=s.device)
+    out_s = torch.full((nq, k), float("-inf"), dtype=torch.float32, device=s.device)
+    m = col.shape[1]
+    out_i[:, :m] = torch.where(present, i.gather(1, col), out_i[:, :m])
+    out_s[:, :m] = torch.where(present, s.gather(1, col), out_s[:, :m])
+    mm = torch.tensor([float("inf"), float("-inf")], device=s.device).repeat(nq, 1)
+    if world:
+        lo, hi = minmax[..., 0].to(torch.float32), minmax[..., 1].to(torch.float32)
+        mm[:, 0] = lo.gather(0, _orderable(lo).argmin(dim=0, keepdim=True))[0]
+        mm[:, 1] = hi.gather(0, _orderable(hi).argmax(dim=0, keepdim=True))[0]
     return out_i, out_s, mm
 
 

@@ -292,7 +292,16 @@ class ShardedIVF:
     """One rank's handle on a row-sharded IVF index (BASELINE config 4 on the GPUs of one box): every rank holds the
     SAME centroid table and the residual lists of its own rows, so all ranks probe the same lists; each searches its
     shard, ONE all-gather of the packed (ids, scores, min/max) records and the merge kernel give every rank the
-    global answer -- the exchange step of the flat row-sharded index (dist.ShardedIndex), unchanged."""
+    global answer -- the exchange step of the flat row-sharded index (dist.ShardedIndex).
+
+    Two consequences of merging per-rank answers (DESIGN.md section 7):
+    * exact ties break by (rank, position in the rank's answer), not by stored position as in one IVFIndex (list,
+      then id): a tie between a lower rank's row in a higher list and a higher rank's row in a lower list goes to the
+      lower rank here, to the lower list there.  The packed record carries no list id, and adding one would grow every
+      exchange of the flat index too;
+    * over a QuantizedIVF each rank keeps its own top `candidates` by S1 and rescores them, so up to world x
+      candidates are rescored.  The answer can differ from one QuantizedIVF over all rows, and its S2 at every
+      position is >= that index's: the global top `candidates` by S1 lie inside the union of the ranks'."""
 
     def __init__(self, local, group=None):
         """`local`: this rank's IVFIndex or QuantizedIVF."""
