@@ -1,5 +1,6 @@
 // Error plumbing, TMA tensor-map construction and device queries for the C ABI.
 #include "common.cuh"
+#include "workspace.cuh"
 
 #include <stdarg.h>
 #include <string.h>
@@ -104,6 +105,13 @@ int sm_count() {
     cached[dev] = n;
   }
   return cached[dev];
+}
+
+int check_workspace(const char* who, const void* ws, size_t bytes, size_t need) {
+  if (!ws) return fail(CRAG_ERR_INVALID, "%s: null workspace pointer", who);
+  if (reinterpret_cast<uintptr_t>(ws) % kWsAlign) return fail(CRAG_ERR_INVALID, "%s: workspace must be 256-byte aligned", who);
+  if (bytes < need) return fail(CRAG_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes", who, bytes, need);
+  return CRAG_OK;
 }
 
 }  // namespace crag

@@ -35,6 +35,10 @@ int make_tmap_u8_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t 
 
 int sm_count();
 
+// A workspace argument (workspace.cuh): CRAG_ERR_INVALID when null or not kWsAlign-aligned, CRAG_ERR_WORKSPACE when
+// `bytes` < `need`; `who` heads the message.
+int check_workspace(const char* who, const void* ws, size_t bytes, size_t need);
+
 // quant.cu.  The address a kernel reads `p` through: device memory as is, page-locked host memory through its device
 // mapping; anything else (pageable host memory) fails with CRAG_ERR_INVALID, `who` heading the message.
 int device_readable(const void* p, const void** out, const char* who);

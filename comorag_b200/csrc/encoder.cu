@@ -9,11 +9,10 @@
 #include "common.cuh"
 #include "encoder.cuh"
 #include "gemm.cuh"
+#include "workspace.cuh"
 
 namespace crag {
 namespace {
-
-inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
 struct EncoderBuffers {
   uint8_t *x, *qkv, *ctx, *tmp, *ff;
@@ -21,16 +20,14 @@ struct EncoderBuffers {
 };
 
 EncoderBuffers carve(void* ws, int T, int H, int I) {
+  WsCursor c(ws);
   EncoderBuffers b;
-  size_t off = 0;
-  uint8_t* base = static_cast<uint8_t*>(ws);
-  auto take = [&](size_t bytes) { uint8_t* p = base ? base + off : nullptr; off += align256(bytes); return p; };
-  b.x = take(size_t(T) * H * 2);
-  b.qkv = take(size_t(T) * 3 * H * 2);
-  b.ctx = take(size_t(T) * H * 2);
-  b.tmp = take(size_t(T) * H * 2);
-  b.ff = take(size_t(T) * I * 2);
-  b.total = off;
+  b.x = c.take<uint8_t>(size_t(T) * H * 2);
+  b.qkv = c.take<uint8_t>(size_t(T) * 3 * H * 2);
+  b.ctx = c.take<uint8_t>(size_t(T) * H * 2);
+  b.tmp = c.take<uint8_t>(size_t(T) * H * 2);
+  b.ff = c.take<uint8_t>(size_t(T) * I * 2);
+  b.total = c.bytes;
   return b;
 }
 
@@ -65,13 +62,13 @@ int run_layers(const crag_encoder* model, const int32_t* token_ids, const int32_
                int total_tokens, int max_seqlen, void* workspace, size_t workspace_bytes, cudaStream_t stream,
                EncoderBuffers& b) {
   if (!token_ids || !cu_seqlens || !workspace) return fail(CRAG_ERR_INVALID, "encoder: null pointer");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "encoder: workspace must be 256-byte aligned");
   if (max_seqlen > model->max_pos - model->pos_offset) return fail(CRAG_ERR_INVALID, "encoder: max_seqlen %d exceeds the position table (%d - %d)", max_seqlen, model->max_pos, model->pos_offset);
   const int T = total_tokens, H = model->hidden, I = model->intermediate;
   b = carve(workspace, T, H, I);
-  if (workspace_bytes < b.total) return fail(CRAG_ERR_WORKSPACE, "encoder: workspace %zu < %zu bytes", workspace_bytes, b.total);
+  int rc = check_workspace("encoder", workspace, workspace_bytes, b.total);
+  if (rc != CRAG_OK) return rc;
 
-  int rc = launch_embed_layernorm(token_ids, cu_seqlens, n_seqs, T, H, model->vocab, model->max_pos, model->pos_offset,
+  rc = launch_embed_layernorm(token_ids, cu_seqlens, n_seqs, T, H, model->vocab, model->max_pos, model->pos_offset,
                                   model->word_emb, model->pos_emb, model->type_emb, model->emb_ln_g, model->emb_ln_b,
                                   model->ln_eps, b.x, stream);
   if (rc != CRAG_OK) return rc;

@@ -50,60 +50,44 @@ extern "C" int crag_gmm_sweep(const double* x, int64_t n, int d, int max_compone
   if (!x || !first_centre || (M > 1 && !seed_draws) || !out_bic || !out_iters || !out_converged || !out_best ||
       !out_weights || !out_means || !out_memberships || !workspace)
     return fail(CRAG_ERR_INVALID, "crag_gmm_sweep: null pointer");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255)
-    return fail(CRAG_ERR_INVALID, "crag_gmm_sweep: workspace must be 256-byte aligned");
-  const GmmPlan p = plan_gmm(n, d, M);
-  if (workspace_bytes < p.total)
-    return fail(CRAG_ERR_WORKSPACE, "crag_gmm_sweep: workspace %zu < %zu bytes", workspace_bytes, p.total);
+  const GmmPlan p = plan_gmm(n, d, M, workspace);
+  const int rc = check_workspace("crag_gmm_sweep", workspace, workspace_bytes, p.total);
+  if (rc != CRAG_OK) return rc;
 
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  double* glob = reinterpret_cast<double*>(ws + p.glob_off);
-  GmmState* state = reinterpret_cast<GmmState*>(ws + p.state_off);
-  double* xc = reinterpret_cast<double*>(ws + p.xc_off);
-  int32_t* labels = out_labels ? out_labels : reinterpret_cast<int32_t*>(ws + p.labels_off);
-  double* dist = reinterpret_cast<double*>(ws + p.dist_off);
-  double* centres = reinterpret_cast<double*>(ws + p.centre_off);
-  double* lsum = reinterpret_cast<double*>(ws + p.lsum_off);
-  int32_t* lchg = reinterpret_cast<int32_t*>(ws + p.lchg_off);
-  double* mu = reinterpret_cast<double*>(ws + p.mu_off);
-  double* prec = reinterpret_cast<double*>(ws + p.prec_off);
-  double* cst = reinterpret_cast<double*>(ws + p.cst_off);
-  double* wt = reinterpret_cast<double*>(ws + p.wt_off);
-  double* esum = reinterpret_cast<double*>(ws + p.esum_off);
-  double* lse = reinterpret_cast<double*>(ws + p.lse_off);
-  int32_t* seeds = out_seeds ? out_seeds : reinterpret_cast<int32_t*>(ws + p.seeds_off);
+  int32_t* labels = out_labels ? out_labels : p.labels;
+  int32_t* seeds = out_seeds ? out_seeds : p.seeds;
   const int R = p.chunks, C = p.components;
   const unsigned grid = unsigned(R) * unsigned(M);
 
-  gmm_moments_kernel<<<1, 1024, sizeof(double) * 1024, stream>>>(x, n, d, M, glob, state);
-  gmm_centre_kernel<<<gmm_blocks(n * (d > M ? d : M), kGmmThreads * 8), kGmmThreads, 0, stream>>>(x, n, d, M, glob, xc,
+  gmm_moments_kernel<<<1, 1024, sizeof(double) * 1024, stream>>>(x, n, d, M, p.glob, p.state);
+  gmm_centre_kernel<<<gmm_blocks(n * (d > M ? d : M), kGmmThreads * 8), kGmmThreads, 0, stream>>>(x, n, d, M, p.glob, p.xc,
                                                                                                   labels);
-  gmm_seed_kernel<<<M, kGmmSeedThreads, kSeedSmem, stream>>>(xc, n, d, first_centre, seed_draws, dist, centres, seeds);
+  gmm_seed_kernel<<<M, kGmmSeedThreads, kSeedSmem, stream>>>(p.xc, n, d, first_centre, seed_draws, p.dist, p.centres, seeds);
   const size_t assign_smem = lloyd_assign_smem(M, d), update_smem = lloyd_update_smem(M, d);
   for (int it = 0; it < kGmmLloydIters; ++it) {
-    gmm_lloyd_assign_kernel<<<grid, kGmmThreads, assign_smem, stream>>>(xc, n, d, M, R, p.chunk_rows, 1, state, centres,
-                                                                       labels, dist, lsum, lchg);
-    gmm_lloyd_update_kernel<<<M, kGmmThreads, update_smem, stream>>>(xc, n, d, M, R, it, glob, state, centres, labels,
-                                                                    dist, lsum, lchg);
+    gmm_lloyd_assign_kernel<<<grid, kGmmThreads, assign_smem, stream>>>(p.xc, n, d, M, R, p.chunk_rows, 1, p.state, p.centres,
+                                                                       labels, p.dist, p.lsum, p.lchg);
+    gmm_lloyd_update_kernel<<<M, kGmmThreads, update_smem, stream>>>(p.xc, n, d, M, R, it, p.glob, p.state, p.centres, labels,
+                                                                    p.dist, p.lsum, p.lchg);
   }
-  gmm_lloyd_assign_kernel<<<grid, kGmmThreads, assign_smem, stream>>>(xc, n, d, M, R, p.chunk_rows, 0, state, centres,
-                                                                     labels, dist, lsum, lchg);
-  gmm_em_setup_kernel<<<gmm_blocks(int64_t(C) * d, kGmmThreads), kGmmThreads, 0, stream>>>(d, C, glob, centres, mu);
+  gmm_lloyd_assign_kernel<<<grid, kGmmThreads, assign_smem, stream>>>(p.xc, n, d, M, R, p.chunk_rows, 0, p.state, p.centres,
+                                                                     labels, p.dist, p.lsum, p.lchg);
+  gmm_em_setup_kernel<<<gmm_blocks(int64_t(C) * d, kGmmThreads), kGmmThreads, 0, stream>>>(d, C, p.glob, p.centres, p.mu);
   const size_t stats_smem = em_stats_smem(M, d), m_smem = mstep_smem(d);
-  gmm_em_stats_kernel<<<grid, kGmmThreads, stats_smem, stream>>>(x, n, d, M, R, p.chunk_rows, kGmmInit, state, nullptr,
-                                                                 labels, mu, prec, cst, esum, lse, nullptr);
-  gmm_mstep_kernel<<<M, kGmmThreads, m_smem, stream>>>(n, d, M, R, kGmmInit, 0, state, mu, prec, cst, wt, esum, lse);
+  gmm_em_stats_kernel<<<grid, kGmmThreads, stats_smem, stream>>>(x, n, d, M, R, p.chunk_rows, kGmmInit, p.state, nullptr,
+                                                                 labels, p.mu, p.prec, p.cst, p.esum, p.lse, nullptr);
+  gmm_mstep_kernel<<<M, kGmmThreads, m_smem, stream>>>(n, d, M, R, kGmmInit, 0, p.state, p.mu, p.prec, p.cst, p.wt, p.esum, p.lse);
   for (int it = 1; it <= kGmmEmIters; ++it) {
-    gmm_em_stats_kernel<<<grid, kGmmThreads, stats_smem, stream>>>(x, n, d, M, R, p.chunk_rows, kGmmStep, state,
-                                                                   nullptr, labels, mu, prec, cst, esum, lse, nullptr);
-    gmm_mstep_kernel<<<M, kGmmThreads, m_smem, stream>>>(n, d, M, R, kGmmStep, it, state, mu, prec, cst, wt, esum, lse);
+    gmm_em_stats_kernel<<<grid, kGmmThreads, stats_smem, stream>>>(x, n, d, M, R, p.chunk_rows, kGmmStep, p.state,
+                                                                   nullptr, labels, p.mu, p.prec, p.cst, p.esum, p.lse, nullptr);
+    gmm_mstep_kernel<<<M, kGmmThreads, m_smem, stream>>>(n, d, M, R, kGmmStep, it, p.state, p.mu, p.prec, p.cst, p.wt, p.esum, p.lse);
   }
-  gmm_em_stats_kernel<<<grid, kGmmThreads, stats_smem, stream>>>(x, n, d, M, R, p.chunk_rows, kGmmScore, state, nullptr,
-                                                                 labels, mu, prec, cst, esum, lse, nullptr);
+  gmm_em_stats_kernel<<<grid, kGmmThreads, stats_smem, stream>>>(x, n, d, M, R, p.chunk_rows, kGmmScore, p.state, nullptr,
+                                                                 labels, p.mu, p.prec, p.cst, p.esum, p.lse, nullptr);
   gmm_select_kernel<<<1, kGmmMaxM, sizeof(double) * (kGmmMaxM + 1), stream>>>(
-      n, d, M, R, state, mu, wt, lse, out_bic, out_iters, out_converged, out_best, out_weights, out_means);
-  gmm_em_stats_kernel<<<unsigned(R), kGmmThreads, stats_smem, stream>>>(x, n, d, M, R, p.chunk_rows, kGmmResp, state,
-                                                                        out_best, labels, mu, prec, cst, esum, lse,
+      n, d, M, R, p.state, p.mu, p.wt, p.lse, out_bic, out_iters, out_converged, out_best, out_weights, out_means);
+  gmm_em_stats_kernel<<<unsigned(R), kGmmThreads, stats_smem, stream>>>(x, n, d, M, R, p.chunk_rows, kGmmResp, p.state,
+                                                                        out_best, labels, p.mu, p.prec, p.cst, p.esum, p.lse,
                                                                         out_memberships);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;

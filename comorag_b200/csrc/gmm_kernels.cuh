@@ -24,6 +24,8 @@
 #include <stdint.h>
 #include <cuda_runtime.h>
 
+#include "workspace.cuh"
+
 #ifndef CRAG_EMULATED_PTX   // tests/warp_emu gives every emulated block its own dynamic shared memory
 #define CRAG_DYNAMIC_SHARED(type, name) extern __shared__ type name[]
 #endif
@@ -58,11 +60,17 @@ struct GmmState {
 struct GmmPlan {
   int chunks, stats, components;                   // row chunks R, statistics per component S, sum of m for m <= M
   int64_t chunk_rows;
-  size_t glob_off, state_off, seeds_off, xc_off, labels_off, dist_off, centre_off, lsum_off, lchg_off, mu_off, prec_off,
-      cst_off, wt_off, esum_off, lse_off, total;
+  double* glob;                                    // the workspace's regions (null when only sized)
+  GmmState* state;
+  int32_t* seeds;                                  // reserved even when the caller takes the seeds
+  double* xc;
+  int32_t* labels;                                 // reserved even when the caller takes the labels
+  double *dist, *centres, *lsum;
+  int32_t* lchg;
+  double *mu, *prec, *cst, *wt, *esum, *lse;
+  size_t total;                                    // workspace bytes
 };
 
-inline size_t gmm_align(size_t b) { return (b + 255) & ~size_t(255); }
 __host__ __device__ inline int64_t gmm_min64(int64_t a, int64_t b) { return a < b ? a : b; }
 __host__ __device__ inline int gmm_tri(int d) { return d * (d + 1) / 2; }
 __host__ __device__ inline int gmm_comp_off(int m) { return m * (m - 1) / 2; }   // model m's first component
@@ -77,7 +85,7 @@ __host__ __device__ inline int64_t gmm_draw_off(int m) {                        
 // centres [C][d], Lloyd chunk sums [R][C][d + 1] and label-change counts int32 [R][M], means [C][d], packed precision
 // Cholesky factors [C][d(d+1)/2], log weight + log det constants [C], weights [C], EM chunk statistics [R][C][S], log-likelihood
 // chunk sums [R][M]; C = M(M+1)/2 components, S = 1 + d + d(d+1)/2.  Nothing scales with n * C.
-inline GmmPlan plan_gmm(int64_t n, int d, int M) {
+inline GmmPlan plan_gmm(int64_t n, int d, int M, void* ws = nullptr) {
   GmmPlan p;
   const int64_t want = (n + kGmmChunkRows - 1) / kGmmChunkRows;
   p.chunks = int(want < 1 ? 1 : want > kGmmMaxChunks ? kGmmMaxChunks : want);
@@ -85,23 +93,23 @@ inline GmmPlan plan_gmm(int64_t n, int d, int M) {
   p.stats = 1 + d + gmm_tri(d);
   p.components = M * (M + 1) / 2;
   const size_t C = size_t(p.components), R = size_t(p.chunks);
-  size_t o = 0;
-  p.glob_off = o;    o += gmm_align(sizeof(double) * (kGmmMaxD + 1));
-  p.state_off = o;   o += gmm_align(sizeof(GmmState) * M);
-  p.seeds_off = o;   o += gmm_align(sizeof(int32_t) * C);
-  p.xc_off = o;      o += gmm_align(sizeof(double) * size_t(n) * d);
-  p.labels_off = o;  o += gmm_align(sizeof(int32_t) * size_t(n) * M);
-  p.dist_off = o;    o += gmm_align(sizeof(double) * size_t(n) * M);
-  p.centre_off = o;  o += gmm_align(sizeof(double) * C * d);
-  p.lsum_off = o;    o += gmm_align(sizeof(double) * R * C * (d + 1));
-  p.lchg_off = o;    o += gmm_align(sizeof(int32_t) * R * M);
-  p.mu_off = o;      o += gmm_align(sizeof(double) * C * d);
-  p.prec_off = o;    o += gmm_align(sizeof(double) * C * gmm_tri(d));
-  p.cst_off = o;     o += gmm_align(sizeof(double) * C);
-  p.wt_off = o;      o += gmm_align(sizeof(double) * C);
-  p.esum_off = o;    o += gmm_align(sizeof(double) * R * C * p.stats);
-  p.lse_off = o;     o += gmm_align(sizeof(double) * R * M);
-  p.total = o;
+  WsCursor c(ws);
+  p.glob = c.take<double>(kGmmMaxD + 1);
+  p.state = c.take<GmmState>(size_t(M));
+  p.seeds = c.take<int32_t>(C);
+  p.xc = c.take<double>(size_t(n) * d);
+  p.labels = c.take<int32_t>(size_t(n) * M);
+  p.dist = c.take<double>(size_t(n) * M);
+  p.centres = c.take<double>(C * d);
+  p.lsum = c.take<double>(R * C * (d + 1));
+  p.lchg = c.take<int32_t>(R * M);
+  p.mu = c.take<double>(C * d);
+  p.prec = c.take<double>(C * gmm_tri(d));
+  p.cst = c.take<double>(C);
+  p.wt = c.take<double>(C);
+  p.esum = c.take<double>(R * C * p.stats);
+  p.lse = c.take<double>(R * M);
+  p.total = c.bytes;
   return p;
 }
 

@@ -37,35 +37,27 @@ extern "C" int crag_ppr(const int64_t* row_ptr, const int32_t* col, const float*
     return fail(CRAG_ERR_INVALID, "crag_ppr: n_out must be >= 0, and equal n_vertices when out_vertices is NULL (%lld)", (long long)n_out);
   if (!row_ptr || !reset || !out || !workspace || (nnz > 0 && (!col || !coef)))
     return fail(CRAG_ERR_INVALID, "crag_ppr: null pointer");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "crag_ppr: workspace must be 256-byte aligned");
-  const PprPlan p = plan_ppr(n, nnz);
-  if (workspace_bytes < p.total) return fail(CRAG_ERR_WORKSPACE, "crag_ppr: workspace %zu < %zu bytes", workspace_bytes, p.total);
+  const PprPlan p = plan_ppr(n, nnz, workspace);
+  const int rc = check_workspace("crag_ppr", workspace, workspace_bytes, p.total);
+  if (rc != CRAG_OK) return rc;
   if (n_out == 0) return CRAG_OK;
-
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  float* y[2] = {reinterpret_cast<float*>(ws), reinterpret_cast<float*>(ws + p.y_bytes)};
-  int32_t* seg_row = reinterpret_cast<int32_t*>(ws + p.seg_row_off);
-  int32_t* head_row = reinterpret_cast<int32_t*>(ws + p.head_row_off);
-  float* head_val = reinterpret_cast<float*>(ws + p.head_val_off);
-  float* carry = reinterpret_cast<float*>(ws + p.carry_off);
-  float* partials = reinterpret_cast<float*>(ws + p.partial_off);
 
   if (iterations > 0)
     ppr_plan_kernel<<<ppr_blocks(p.segments + 1, kPprThreads), kPprThreads, 0, stream>>>(row_ptr, n, nnz, p.segments,
-                                                                                        seg_row, head_row);
-  ppr_init_kernel<<<ppr_blocks(n, kPprThreads), kPprThreads, 0, stream>>>(reset, damping, n, y[0]);
+                                                                                        p.seg_row, p.head_row);
+  ppr_init_kernel<<<ppr_blocks(n, kPprThreads), kPprThreads, 0, stream>>>(reset, damping, n, p.y[0]);
   for (int t = 0; t < iterations; ++t) {
-    const float* y_in = y[t & 1];
-    float* y_out = y[(t + 1) & 1];
+    const float* y_in = p.y[t & 1];
+    float* y_out = p.y[(t + 1) & 1];
     ppr_step_kernel<<<ppr_blocks(p.segments, kPprStepWarps), kPprStepThreads, kPprStepSmemBytes, stream>>>(
-        row_ptr, col, coef, reset, damping, y_in, y_out, seg_row, head_row, n, nnz, p.segments, head_val, carry);
-    ppr_fixup_kernel<<<ppr_blocks(p.segments, kPprThreads), kPprThreads, 0, stream>>>(row_ptr, reset, damping, head_row,
-                                                                                     head_val, carry, p.segments, y_out);
+        row_ptr, col, coef, reset, damping, y_in, y_out, p.seg_row, p.head_row, n, nnz, p.segments, p.head_val, p.carry);
+    ppr_fixup_kernel<<<ppr_blocks(p.segments, kPprThreads), kPprThreads, 0, stream>>>(row_ptr, reset, damping, p.head_row,
+                                                                                     p.head_val, p.carry, p.segments, y_out);
   }
-  const float* y_T = y[iterations & 1];
-  ppr_sum_kernel<<<p.sum_blocks, kPprThreads, kPprSumSmemBytes, stream>>>(y_T, n, partials);
+  const float* y_T = p.y[iterations & 1];
+  ppr_sum_kernel<<<p.sum_blocks, kPprThreads, kPprSumSmemBytes, stream>>>(y_T, n, p.partials);
   ppr_gather_kernel<<<ppr_blocks(n_out, kPprThreads), kPprThreads, kPprSumSmemBytes, stream>>>(
-      y_T, partials, p.sum_blocks, out_vertices, n_out, out);
+      y_T, p.partials, p.sum_blocks, out_vertices, n_out, out);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }
@@ -74,35 +66,26 @@ namespace {
 template <int W>
 void launch_ppr_batch(const PprBatchPlan& p, const int64_t* row_ptr, const int32_t* col, const float* coef, int64_t n,
                       int64_t nnz, const float* resets, int batch, float damping, int iterations,
-                      const int32_t* out_vertices, int64_t n_out, float* out, uint8_t* ws, cudaStream_t stream) {
-  float* y[2] = {reinterpret_cast<float*>(ws), reinterpret_cast<float*>(ws + p.y_bytes)};
-  float* v = reinterpret_cast<float*>(ws + p.v_off);
-  int32_t* seg_row = reinterpret_cast<int32_t*>(ws + p.seg_row_off);
-  int32_t* head_row = reinterpret_cast<int32_t*>(ws + p.head_row_off);
-  float* head_val = reinterpret_cast<float*>(ws + p.head_val_off);
-  float* carry = reinterpret_cast<float*>(ws + p.carry_off);
-  float* partials = reinterpret_cast<float*>(ws + p.partial_off);
-  float* totals = reinterpret_cast<float*>(ws + p.total_off);
-
+                      const int32_t* out_vertices, int64_t n_out, float* out, cudaStream_t stream) {
   if (iterations > 0)
     ppr_plan_kernel<<<ppr_blocks(p.segments + 1, kPprThreads), kPprThreads, 0, stream>>>(row_ptr, n, nnz, p.segments,
-                                                                                        seg_row, head_row);
-  ppr_batch_init_kernel<W><<<ppr_blocks(n * W, kPprThreads), kPprThreads, 0, stream>>>(resets, batch, damping, n, v,
-                                                                                       y[0]);
+                                                                                        p.seg_row, p.head_row);
+  ppr_batch_init_kernel<W><<<ppr_blocks(n * W, kPprThreads), kPprThreads, 0, stream>>>(resets, batch, damping, n, p.v,
+                                                                                       p.y[0]);
   for (int t = 0; t < iterations; ++t) {
-    const float* y_in = y[t & 1];
-    float* y_out = y[(t + 1) & 1];
+    const float* y_in = p.y[t & 1];
+    float* y_out = p.y[(t + 1) & 1];
     ppr_batch_step_kernel<W><<<ppr_blocks(p.segments, kPprStepWarps), kPprStepThreads, kPprBatchStepSmemBytes, stream>>>(
-        row_ptr, col, coef, v, damping, y_in, y_out, seg_row, head_row, n, nnz, p.segments, head_val, carry);
+        row_ptr, col, coef, p.v, damping, y_in, y_out, p.seg_row, p.head_row, n, nnz, p.segments, p.head_val, p.carry);
     ppr_batch_fixup_kernel<W><<<ppr_blocks(p.segments * W, kPprThreads), kPprThreads, 0, stream>>>(
-        row_ptr, v, damping, head_row, head_val, carry, p.segments, y_out);
+        row_ptr, p.v, damping, p.head_row, p.head_val, p.carry, p.segments, y_out);
   }
-  const float* y_T = y[iterations & 1];
-  ppr_batch_sum_kernel<W><<<p.sum_blocks, kPprThreads, kPprSumSmemBytes, stream>>>(y_T, n, partials);
-  ppr_batch_total_kernel<W><<<W, kPprThreads, kPprSumSmemBytes, stream>>>(partials, p.sum_blocks, totals);
+  const float* y_T = p.y[iterations & 1];
+  ppr_batch_sum_kernel<W><<<p.sum_blocks, kPprThreads, kPprSumSmemBytes, stream>>>(y_T, n, p.partials);
+  ppr_batch_total_kernel<W><<<W, kPprThreads, kPprSumSmemBytes, stream>>>(p.partials, p.sum_blocks, p.totals);
   const int64_t per_column = ppr_blocks(n_out, kPprThreads);
-  ppr_batch_gather_kernel<W><<<unsigned(per_column * batch), kPprThreads, 0, stream>>>(y_T, totals, out_vertices, n_out,
-                                                                                      per_column, out);
+  ppr_batch_gather_kernel<W><<<unsigned(per_column * batch), kPprThreads, 0, stream>>>(y_T, p.totals, out_vertices,
+                                                                                      n_out, per_column, out);
 }
 }  // namespace
 
@@ -130,20 +113,17 @@ extern "C" int crag_ppr_batch(const int64_t* row_ptr, const int32_t* col, const 
     return fail(CRAG_ERR_INVALID, "crag_ppr_batch: n_out must be >= 0, and equal n_vertices when out_vertices is NULL (%lld)", (long long)n_out);
   if (!row_ptr || !resets || !out || !workspace || (nnz > 0 && (!col || !coef)))
     return fail(CRAG_ERR_INVALID, "crag_ppr_batch: null pointer");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255)
-    return fail(CRAG_ERR_INVALID, "crag_ppr_batch: workspace must be 256-byte aligned");
-  const PprBatchPlan p = plan_ppr_batch(n, nnz, batch);
-  if (workspace_bytes < p.total)
-    return fail(CRAG_ERR_WORKSPACE, "crag_ppr_batch: workspace %zu < %zu bytes", workspace_bytes, p.total);
+  const PprBatchPlan p = plan_ppr_batch(n, nnz, batch, workspace);
+  const int rc = check_workspace("crag_ppr_batch", workspace, workspace_bytes, p.total);
+  if (rc != CRAG_OK) return rc;
   if (n_out == 0) return CRAG_OK;
 
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
   switch (p.width) {
-    case 2: launch_ppr_batch<2>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, ws, stream); break;
-    case 4: launch_ppr_batch<4>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, ws, stream); break;
-    case 8: launch_ppr_batch<8>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, ws, stream); break;
-    case 16: launch_ppr_batch<16>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, ws, stream); break;
-    default: launch_ppr_batch<32>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, ws, stream); break;
+    case 2: launch_ppr_batch<2>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, stream); break;
+    case 4: launch_ppr_batch<4>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, stream); break;
+    case 8: launch_ppr_batch<8>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, stream); break;
+    case 16: launch_ppr_batch<16>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, stream); break;
+    default: launch_ppr_batch<32>(p, row_ptr, col, coef, n, nnz, resets, batch, damping, iterations, out_vertices, n_out, out, stream); break;
   }
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;

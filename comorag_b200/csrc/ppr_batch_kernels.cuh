@@ -42,27 +42,33 @@ struct PprBatchPlan {
   int64_t segments;                                // as plan_ppr
   int sum_blocks;
   int width;
-  size_t y_bytes, v_off, seg_row_off, head_row_off, head_val_off, carry_off, partial_off, total_off, total;
+  float* y[2];                                     // the workspace's regions (null when only sized)
+  float* v;
+  int32_t *seg_row, *head_row;
+  float *head_val, *carry, *partials, *totals;
+  size_t total;                                    // workspace bytes
 };
 
-// Workspace: y[2][n][W] fp32, the resets transposed to v[n][W], seg_row and head_row as crag_ppr, head_val and carry
-// fp32 [segments][W], partial sums fp32 [sum_blocks][W], totals fp32 [W]; every part 256-B aligned.
-inline PprBatchPlan plan_ppr_batch(int64_t n, int64_t nnz, int batch) {
+// Workspace `ws`: y[2][n][W] fp32, the resets transposed to v[n][W], seg_row and head_row as crag_ppr, head_val and
+// carry fp32 [segments][W], partial sums fp32 [sum_blocks][W], totals fp32 [W].
+inline PprBatchPlan plan_ppr_batch(int64_t n, int64_t nnz, int batch, void* ws = nullptr) {
   const PprPlan single = plan_ppr(n, nnz);
   PprBatchPlan p;
   p.segments = single.segments;
   p.sum_blocks = single.sum_blocks;
   p.width = ppr_batch_width(batch);
   const size_t W = size_t(p.width);
-  p.y_bytes = ppr_align(size_t(n) * W * 4);
-  p.v_off = 2 * p.y_bytes;
-  p.seg_row_off = p.v_off + p.y_bytes;
-  p.head_row_off = p.seg_row_off + ppr_align(size_t(p.segments + 1) * 4);
-  p.head_val_off = p.head_row_off + ppr_align(size_t(p.segments) * 4);
-  p.carry_off = p.head_val_off + ppr_align(size_t(p.segments) * W * 4);
-  p.partial_off = p.carry_off + ppr_align(size_t(p.segments) * W * 4);
-  p.total_off = p.partial_off + ppr_align(size_t(p.sum_blocks) * W * 4);
-  p.total = p.total_off + ppr_align(W * 4);
+  WsCursor c(ws);
+  p.y[0] = c.take<float>(size_t(n) * W);
+  p.y[1] = c.take<float>(size_t(n) * W);
+  p.v = c.take<float>(size_t(n) * W);
+  p.seg_row = c.take<int32_t>(size_t(p.segments + 1));
+  p.head_row = c.take<int32_t>(size_t(p.segments));
+  p.head_val = c.take<float>(size_t(p.segments) * W);
+  p.carry = c.take<float>(size_t(p.segments) * W);
+  p.partials = c.take<float>(size_t(p.sum_blocks) * W);
+  p.totals = c.take<float>(W);
+  p.total = c.bytes;
   return p;
 }
 

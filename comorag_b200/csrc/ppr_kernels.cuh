@@ -21,6 +21,8 @@
 #include <stdint.h>
 #include <cuda_runtime.h>
 
+#include "workspace.cuh"
+
 #ifndef CRAG_EMULATED_PTX   // tests/warp_emu gives every emulated block its own dynamic shared memory
 #define CRAG_DYNAMIC_SHARED(type, name) extern __shared__ type name[]
 #endif
@@ -40,25 +42,28 @@ constexpr size_t kPprSumSmemBytes = size_t(kPprThreads) * 4;
 struct PprPlan {
   int64_t segments;                                // ceil((n + nnz) / kPprSegItems)
   int sum_blocks;
-  size_t y_bytes, seg_row_off, head_row_off, head_val_off, carry_off, partial_off, total;
+  float* y[2];                                     // the workspace's regions (null when only sized)
+  int32_t *seg_row, *head_row;
+  float *head_val, *carry, *partials;
+  size_t total;                                    // workspace bytes
 };
 
-inline size_t ppr_align(size_t b) { return (b + 255) & ~size_t(255); }
-
-// Workspace: y[2][n] fp32 (double buffer), seg_row int32 [segments + 1], head_row int32, head_val and carry fp32
-// [segments], partial sums fp32 [sum_blocks]; every part 256-B aligned.
-inline PprPlan plan_ppr(int64_t n, int64_t nnz) {
+// Workspace `ws`: y[2][n] fp32 (double buffer), seg_row int32 [segments + 1], head_row int32, head_val and carry fp32
+// [segments], partial sums fp32 [sum_blocks].
+inline PprPlan plan_ppr(int64_t n, int64_t nnz, void* ws = nullptr) {
   PprPlan p;
   p.segments = (n + nnz + kPprSegItems - 1) / kPprSegItems;
   const int64_t blocks = (n + kPprThreads - 1) / kPprThreads;
   p.sum_blocks = int(blocks < 1 ? 1 : blocks > kPprMaxSumBlocks ? kPprMaxSumBlocks : blocks);
-  p.y_bytes = ppr_align(size_t(n) * 4);
-  p.seg_row_off = 2 * p.y_bytes;
-  p.head_row_off = p.seg_row_off + ppr_align(size_t(p.segments + 1) * 4);
-  p.head_val_off = p.head_row_off + ppr_align(size_t(p.segments) * 4);
-  p.carry_off = p.head_val_off + ppr_align(size_t(p.segments) * 4);
-  p.partial_off = p.carry_off + ppr_align(size_t(p.segments) * 4);
-  p.total = p.partial_off + ppr_align(size_t(p.sum_blocks) * 4);
+  WsCursor c(ws);
+  p.y[0] = c.take<float>(size_t(n));
+  p.y[1] = c.take<float>(size_t(n));
+  p.seg_row = c.take<int32_t>(size_t(p.segments + 1));
+  p.head_row = c.take<int32_t>(size_t(p.segments));
+  p.head_val = c.take<float>(size_t(p.segments));
+  p.carry = c.take<float>(size_t(p.segments));
+  p.partials = c.take<float>(size_t(p.sum_blocks));
+  p.total = c.bytes;
   return p;
 }
 

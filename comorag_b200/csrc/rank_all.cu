@@ -29,20 +29,17 @@ extern "C" int crag_rank_scores(const float* scores, int64_t n, int64_t* out_ids
   if (n < 0 || n >= (int64_t(1) << 31)) return fail(CRAG_ERR_INVALID, "crag_rank_scores: n out of range (%lld)", (long long)n);
   if (n == 0) return CRAG_OK;
   if (!scores || !out_ids || !out_scores || !workspace) return fail(CRAG_ERR_INVALID, "crag_rank_scores: null pointer");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "crag_rank_scores: workspace must be 256-byte aligned");
-  const SortPlan p = plan_sort(n);
-  if (workspace_bytes < p.total) return fail(CRAG_ERR_WORKSPACE, "crag_rank_scores: workspace %zu < %zu bytes", workspace_bytes, p.total);
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  uint32_t* keys[2] = {reinterpret_cast<uint32_t*>(ws), reinterpret_cast<uint32_t*>(ws + p.key_bytes)};
-  uint32_t* vals[2] = {reinterpret_cast<uint32_t*>(ws + 2 * p.key_bytes), reinterpret_cast<uint32_t*>(ws + 2 * p.key_bytes + p.val_bytes)};
-  uint32_t* hist = reinterpret_cast<uint32_t*>(ws + 2 * p.key_bytes + 2 * p.val_bytes);
+  const SortPlan p = plan_sort(n, workspace);
+  const int rc = check_workspace("crag_rank_scores", workspace, workspace_bytes, p.total);
+  if (rc != CRAG_OK) return rc;
+  uint32_t* hist = p.hist;
   uint32_t* totals = hist + size_t(256) * p.n_warps;
   for (int pass = 0; pass < 4; ++pass) {
     const int shift = pass * 8;
-    const uint32_t* kin = pass ? keys[(pass - 1) & 1] : nullptr;
-    const uint32_t* vin = pass ? vals[(pass - 1) & 1] : nullptr;
-    uint32_t* kout = keys[pass & 1];
-    uint32_t* vout = vals[pass & 1];
+    const uint32_t* kin = pass ? p.keys[(pass - 1) & 1] : nullptr;
+    const uint32_t* vin = pass ? p.vals[(pass - 1) & 1] : nullptr;
+    uint32_t* kout = p.keys[pass & 1];
+    uint32_t* vout = p.vals[pass & 1];
     CRAG_CUDA_OK(cudaMemsetAsync(totals, 0, 256 * 4, stream));
     if (pass == 0) hist_kernel<true><<<p.grid, kSortThreads, 0, stream>>>(scores, nullptr, n, p.run, p.n_warps, shift, hist, totals);
     else hist_kernel<false><<<p.grid, kSortThreads, 0, stream>>>(nullptr, kin, n, p.run, p.n_warps, shift, hist, totals);

@@ -7,6 +7,7 @@
 #include <cuda_runtime.h>
 
 #include "topk.cuh"
+#include "workspace.cuh"
 
 namespace crag {
 namespace {
@@ -18,10 +19,12 @@ struct SortPlan {
   int run;         // elements per warp (multiple of 32)
   int n_warps;     // total warps
   int grid;
-  size_t key_bytes, val_bytes, hist_bytes, total;
+  uint32_t *keys[2], *vals[2];   // the workspace's double buffers (null when only sized)
+  uint32_t* hist;                // [256][n_warps] digit counts, then the 256 digit totals
+  size_t total;                  // workspace bytes
 };
 
-SortPlan plan_sort(int64_t n) {
+SortPlan plan_sort(int64_t n, void* ws = nullptr) {
   SortPlan p;
   // runs of 2048 elements; for big arrays grow the run so the histogram table stays small (<= 8192 warps)
   int64_t run = 2048;
@@ -30,11 +33,13 @@ SortPlan plan_sort(int64_t n) {
   p.n_warps = int((n + run - 1) / run);
   if (p.n_warps < 1) p.n_warps = 1;
   p.grid = (p.n_warps + kWarpsPerCta - 1) / kWarpsPerCta;
-  auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
-  p.key_bytes = up(size_t(n) * 4);
-  p.val_bytes = up(size_t(n) * 4);
-  p.hist_bytes = up(size_t(256) * p.n_warps * 4 + 256 * 4);
-  p.total = 2 * p.key_bytes + 2 * p.val_bytes + p.hist_bytes;
+  WsCursor c(ws);
+  p.keys[0] = c.take<uint32_t>(size_t(n));
+  p.keys[1] = c.take<uint32_t>(size_t(n));
+  p.vals[0] = c.take<uint32_t>(size_t(n));
+  p.vals[1] = c.take<uint32_t>(size_t(n));
+  p.hist = c.take<uint32_t>(size_t(256) * p.n_warps + 256);
+  p.total = c.bytes;
   return p;
 }
 

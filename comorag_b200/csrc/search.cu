@@ -44,6 +44,7 @@
 #include "select_warps.cuh"
 #include "gemm.cuh"
 #include "knn_select.cuh"
+#include "workspace.cuh"
 
 namespace crag {
 
@@ -252,20 +253,31 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
 // ------------------------------------------------------------------ host side
 namespace {
 
+// Workspace of a flat scan, per 32-query pass: the per-CTA partial keys and (min, max), then the pooled-floor table
+// (0 bytes when the grid exceeds kPoolMaxCtas).  Every scan needs the partials; a flat scan uses the table if it fits.
 struct SearchPlan {
   int grid;
-  size_t keys_bytes;    // per 32-query pass
-  size_t minmax_bytes;  // per 32-query pass
-  size_t pool_bytes;    // pooled-floor table of one 32-query pass (0 when the grid exceeds kPoolMaxCtas)
+  uint64_t* part_keys;
+  float* part_minmax;
+  size_t parts_bytes;
+  uint64_t* pool;       // null without a table
+  size_t pool_bytes;
+  size_t total;
 };
 
-SearchPlan plan_search(int k) {
+SearchPlan plan_search(int k, const void* ws = nullptr) {
   SearchPlan p;
   p.grid = sm_count();
   if (p.grid <= 0) p.grid = 132;
-  p.keys_bytes = ((size_t(p.grid) * kNQ * k * 8) + 255) & ~size_t(255);
-  p.minmax_bytes = ((size_t(p.grid) * kNQ * 2 * 4) + 255) & ~size_t(255);
-  p.pool_bytes = p.grid <= kPoolMaxCtas ? ((size_t(kNQ) * p.grid * kPoolSlots * 8 + 255) & ~size_t(255)) : 0;
+  WsCursor c(ws);
+  p.part_keys = c.take<uint64_t>(size_t(p.grid) * kNQ * k);
+  p.part_minmax = c.take<float>(size_t(p.grid) * kNQ * 2);
+  p.parts_bytes = c.bytes;
+  const bool pooled = p.grid <= kPoolMaxCtas;
+  uint64_t* pool = c.take<uint64_t>(pooled ? size_t(kNQ) * p.grid * kPoolSlots : 0);
+  p.pool = pooled ? pool : nullptr;
+  p.pool_bytes = c.bytes - p.parts_bytes;
+  p.total = c.bytes;
   return p;
 }
 
@@ -343,10 +355,7 @@ int check_scan_args(const char* who, int nq, int k, int k_max, const Operand& co
   int rc = check_operand(who, corpus);
   if (rc == CRAG_OK) rc = check_operand(who, queries);
   if (rc != CRAG_OK) return rc;
-  if (!workspace) return fail(CRAG_ERR_INVALID, "%s: null workspace pointer", who);
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail(CRAG_ERR_INVALID, "%s: workspace must be 256-byte aligned", who);
-  if (workspace_bytes < need) return fail(CRAG_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes", who, workspace_bytes, need);
-  return CRAG_OK;
+  return check_workspace(who, workspace, workspace_bytes, need);
 }
 
 // TMA map of an operand in boxes of box_rows rows by one 128-byte swizzle row
@@ -363,8 +372,7 @@ using namespace crag;
 extern "C" size_t crag_search_workspace_bytes(int nq, int k) {
   (void)nq;
   if (k < 1 || k > 128) return 0;
-  const SearchPlan p = plan_search(k);
-  return p.keys_bytes + p.minmax_bytes + p.pool_bytes;
+  return plan_search(k).total;
 }
 
 namespace crag {
@@ -381,16 +389,14 @@ constexpr int kPermShift = 3;
 // one corpus pass for the <= 32 queries of `queries`: per-CTA partial lists into the workspace
 template <class Args>
 int scan_pass(const Operand& corpus, const Operand& queries, int k, const uint64_t* after_keys, const Args& args,
-              void* workspace, size_t workspace_bytes, const SearchPlan& plan, cudaStream_t stream) {
+              size_t workspace_bytes, const SearchPlan& plan, cudaStream_t stream) {
   const int grid = scan_grid(corpus.rows, plan);
   if (grid == 0) return CRAG_OK;
-  uint64_t* part_keys = static_cast<uint64_t*>(workspace);
-  float* part_minmax = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + plan.keys_bytes);
   // pooled floor: needs its table in the workspace and pays off once a CTA sees more than a couple of tiles
   uint64_t* pool = nullptr;
   const int64_t num_tiles = (corpus.rows + kTileRows - 1) / kTileRows;
-  if (plan.pool_bytes && workspace_bytes >= plan.keys_bytes + plan.minmax_bytes + plan.pool_bytes && num_tiles >= 4 * int64_t(grid)) {
-    pool = reinterpret_cast<uint64_t*>(static_cast<uint8_t*>(workspace) + plan.keys_bytes + plan.minmax_bytes);
+  if (plan.pool && workspace_bytes >= plan.total && num_tiles >= 4 * int64_t(grid)) {
+    pool = plan.pool;
     CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, plan.pool_bytes, stream));
   }
   CUtensorMap tm_corpus, tm_q;
@@ -398,17 +404,15 @@ int scan_pass(const Operand& corpus, const Operand& queries, int k, const uint64
   if (rc == CRAG_OK) rc = make_tmap(&tm_q, queries, kNQ);
   if (rc != CRAG_OK) return rc;
   return launch_topk_scan(tm_corpus, tm_q, int(corpus.rows), corpus.num_kb(), int(queries.rows), k, grid, after_keys, pool,
-                          perm_multiplier(num_tiles >> kPermShift), kPermShift, part_keys, part_minmax, args, stream);
+                          perm_multiplier(num_tiles >> kPermShift), kPermShift, plan.part_keys, plan.part_minmax, args, stream);
 }
 
 // merge the per-CTA partials of one pass into the final (ids, scores, minmax) of its <= 32 queries
-int finalize_parts(const void* workspace, int grid, int nq, int k, int64_t row_offset, int64_t* out_ids,
-                   float* out_scores, float* out_minmax, uint64_t* last_keys, const SearchPlan& plan, cudaStream_t stream) {
-  const uint64_t* part_keys = static_cast<const uint64_t*>(workspace);
-  const float* part_minmax = reinterpret_cast<const float*>(static_cast<const uint8_t*>(workspace) + plan.keys_bytes);
+int finalize_parts(int grid, int nq, int k, int64_t row_offset, int64_t* out_ids, float* out_scores, float* out_minmax,
+                   uint64_t* last_keys, const SearchPlan& plan, cudaStream_t stream) {
   with_merge_tier(k, [&](auto tier) {   // one CTA per query
     constexpr int T = decltype(tier)::value;
-    merge_topk_kernel<T, T, false><<<nq, 128, 0, stream>>>(part_keys, nullptr, nullptr, part_minmax, grid, kNQ, nq, k, row_offset, 0, 0, 0,
+    merge_topk_kernel<T, T, false><<<nq, 128, 0, stream>>>(plan.part_keys, nullptr, nullptr, plan.part_minmax, grid, kNQ, nq, k, row_offset, 0, 0, 0,
                                                            out_ids, out_scores, out_minmax, last_keys);
   });
   CRAG_CUDA_OK(cudaGetLastError());
@@ -419,46 +423,55 @@ int finalize_parts(const void* workspace, int grid, int nq, int k, int64_t row_o
 template <class Args>
 int topk_passes(const Operand& corpus, const Operand& queries, int k, int64_t row_offset, const uint64_t* after_keys,
                 const Args& args, int64_t* out_ids, float* out_scores, float* out_minmax, uint64_t* last_keys,
-                void* workspace, size_t workspace_bytes, const SearchPlan& plan, cudaStream_t stream) {
+                size_t workspace_bytes, const SearchPlan& plan, cudaStream_t stream) {
   const int nq = int(queries.rows);
   for (int q0 = 0; q0 < nq; q0 += kNQ) {
     const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
     int rc = scan_pass(corpus, queries.rows_from(q0, nqc), k, after_keys ? after_keys + q0 : nullptr, pass_args(args, q0),
-                       workspace, workspace_bytes, plan, stream);
+                       workspace_bytes, plan, stream);
     if (rc == CRAG_OK)
-      rc = finalize_parts(workspace, scan_grid(corpus.rows, plan), nqc, k, row_offset, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
+      rc = finalize_parts(scan_grid(corpus.rows, plan), nqc, k, row_offset, out_ids + size_t(q0) * k, out_scores + size_t(q0) * k,
                          out_minmax ? out_minmax + size_t(q0) * 2 : nullptr, last_keys ? last_keys + q0 : nullptr, plan, stream);
     if (rc != CRAG_OK) return rc;
   }
   return CRAG_OK;
 }
 
-// IVF workspace = the flat scan's per-CTA partials, then the per-pass plan
+// IVF workspace = the flat scan's, then the per-pass plan of the probed tiles
 struct IvfPlan {
-  size_t pool_off, mask_off, coarse_off, work_off, count_off, total;
+  SearchPlan scan;
+  uint32_t* list_mask;
+  float* coarse;
+  int4* work;
+  int* n_work;
+  size_t total;
 };
-IvfPlan plan_ivf(const SearchPlan& sp, int nlist, int64_t total_tiles) {
-  auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
+IvfPlan plan_ivf(int k, int nlist, int64_t total_tiles, const void* ws = nullptr) {
   IvfPlan p;
-  p.pool_off = sp.keys_bytes + sp.minmax_bytes;
-  p.mask_off = p.pool_off + sp.pool_bytes;
-  p.coarse_off = p.mask_off + up(size_t(nlist) * 4);
-  p.work_off = p.coarse_off + up(size_t(nlist) * kNQ * 4);
-  p.count_off = p.work_off + up(size_t(total_tiles) * sizeof(int4));
-  p.total = p.count_off + 256;
+  p.scan = plan_search(k, ws);
+  WsCursor c(ws, p.scan.total);
+  p.list_mask = c.take<uint32_t>(size_t(nlist));
+  p.coarse = c.take<float>(size_t(nlist) * kNQ);
+  p.work = c.take<int4>(size_t(total_tiles));
+  p.n_work = c.take<int>(1);
+  p.total = c.bytes;
   return p;
 }
 
+// int8 IVF workspace = the IVF workspace for n_cand keys, then the candidates of one pass
 struct IvfI8Plan {
   IvfPlan ivf;
-  size_t cand_ids_off, cand_scores_off, total;
+  int64_t* cand_ids;
+  float* cand_scores;
+  size_t total;
 };
-IvfI8Plan plan_ivf_i8(int nlist, int64_t total_tiles, int n_cand) {
+IvfI8Plan plan_ivf_i8(int nlist, int64_t total_tiles, int n_cand, const void* ws = nullptr) {
   IvfI8Plan p;
-  p.ivf = plan_ivf(plan_search(n_cand), nlist, total_tiles);
-  p.cand_ids_off = p.ivf.total;
-  p.cand_scores_off = p.cand_ids_off + ((size_t(kNQ) * n_cand * 8 + 255) & ~size_t(255));
-  p.total = p.cand_scores_off + ((size_t(kNQ) * n_cand * 4 + 255) & ~size_t(255));
+  p.ivf = plan_ivf(n_cand, nlist, total_tiles, ws);
+  WsCursor c(ws, p.ivf.total);
+  p.cand_ids = c.take<int64_t>(size_t(kNQ) * n_cand);
+  p.cand_scores = c.take<float>(size_t(kNQ) * n_cand);
+  p.total = c.bytes;
   return p;
 }
 
@@ -493,16 +506,10 @@ struct IvfRescore {
 // writes n_scan candidates, which the exact rescore (quant.cu) turns into the k results, with the plan's coarse terms.
 template <class Args>
 int ivf_passes(const Operand& res, const Operand& queries, Args args, const IvfLists& l, int n_scan, int k,
-               const IvfRescore* rescore, int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
-               const IvfPlan& ip, const SearchPlan& sp, cudaStream_t stream) {
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  uint64_t* part_keys = reinterpret_cast<uint64_t*>(ws);
-  float* part_minmax = reinterpret_cast<float*>(ws + sp.keys_bytes);
-  uint32_t* list_mask = reinterpret_cast<uint32_t*>(ws + ip.mask_off);
-  float* coarse = reinterpret_cast<float*>(ws + ip.coarse_off);
-  int4* work = reinterpret_cast<int4*>(ws + ip.work_off);
-  int* n_work = reinterpret_cast<int*>(ws + ip.count_off);
-  static_cast<IvfArgs&>(args) = IvfArgs{work, n_work, list_mask, coarse};
+               const IvfRescore* rescore, int64_t* out_ids, float* out_scores, float* out_minmax, const IvfPlan& ip,
+               cudaStream_t stream) {
+  const SearchPlan& sp = ip.scan;
+  static_cast<IvfArgs&>(args) = IvfArgs{ip.work, ip.n_work, ip.list_mask, ip.coarse};
   CUtensorMap tm_res;
   int rc = make_tmap(&tm_res, res, kTileRows);
   if (rc != CRAG_OK) return rc;
@@ -513,28 +520,25 @@ int ivf_passes(const Operand& res, const Operand& queries, Args args, const IvfL
     rc = make_tmap(&tm_q, queries.rows_from(q0, nqc), kNQ);
     if (rc != CRAG_OK) return rc;
     ivf_plan_kernel<<<1, 1024, 0, stream>>>(l.probed_ids + size_t(q0) * l.nprobe, l.probed_scores + size_t(q0) * l.nprobe, nqc,
-                                            l.nprobe, l.nlist, l.tile_start, l.rows, list_mask, coarse, work, n_work);
+                                            l.nprobe, l.nlist, l.tile_start, l.rows, ip.list_mask, ip.coarse, ip.work,
+                                            ip.n_work);
     CRAG_CUDA_OK(cudaGetLastError());
     // every CTA of the grid publishes a (possibly empty) partial list, so the merge always reads sp.grid parts
-    uint64_t* pool = nullptr;
-    if (sp.pool_bytes) {
-      pool = reinterpret_cast<uint64_t*>(ws + ip.pool_off);
-      CRAG_CUDA_OK(cudaMemsetAsync(pool, 0, sp.pool_bytes, stream));
-    }
-    rc = launch_topk_scan(tm_res, tm_q, int(res.rows), res.num_kb(), nqc, n_scan, sp.grid, nullptr, pool, 0u, 0,
-                          part_keys, part_minmax, pass_args(args, q0), stream);
+    if (sp.pool) CRAG_CUDA_OK(cudaMemsetAsync(sp.pool, 0, sp.pool_bytes, stream));
+    rc = launch_topk_scan(tm_res, tm_q, int(res.rows), res.num_kb(), nqc, n_scan, sp.grid, nullptr, sp.pool, 0u, 0,
+                          sp.part_keys, sp.part_minmax, pass_args(args, q0), stream);
     if (rc != CRAG_OK) return rc;
     int64_t* ids = out_ids + size_t(q0) * k;
     float* scores = out_scores + size_t(q0) * k;
     float* minmax = out_minmax ? out_minmax + size_t(q0) * 2 : nullptr;
     if (!rescore) {
-      rc = finalize_parts(workspace, sp.grid, nqc, k, 0, ids, scores, minmax, nullptr, sp, stream);
+      rc = finalize_parts(sp.grid, nqc, k, 0, ids, scores, minmax, nullptr, sp, stream);
     } else {
-      rc = finalize_parts(workspace, sp.grid, nqc, n_scan, 0, rescore->cand_ids, rescore->cand_scores, minmax, nullptr, sp, stream);
+      rc = finalize_parts(sp.grid, nqc, n_scan, 0, rescore->cand_ids, rescore->cand_scores, minmax, nullptr, sp, stream);
       if (rc == CRAG_OK)
         rc = launch_ivf_rescore(rescore->rows.ptr, rescore->rows.rows, rescore->rows.width, rescore->rows.stride,
                                 rescore->queries.rows_from(q0, nqc).ptr, nqc, rescore->cand_ids, n_scan, k, l.tile_start,
-                                l.nlist, coarse, ids, scores, stream);
+                                l.nlist, ip.coarse, ids, scores, stream);
     }
     if (rc != CRAG_OK) return rc;
     ivf_map_ids_kernel<<<(nqc * k + 255) / 256, 256, 0, stream>>>(ids, nqc * k, l.row_ids);
@@ -548,7 +552,7 @@ int ivf_passes(const Operand& res, const Operand& queries, Args args, const IvfL
 
 extern "C" size_t crag_ivf_workspace_bytes(int nlist, int64_t total_tiles, int k) {
   if (nlist < 1 || total_tiles < 0 || k < 1 || k > 128) return 0;
-  return plan_ivf(plan_search(k), nlist, total_tiles).total;
+  return plan_ivf(k, nlist, total_tiles).total;
 }
 
 extern "C" int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int dim, int64_t row_stride,
@@ -561,11 +565,10 @@ extern "C" int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int
   const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
   int rc = check_ivf_args("ivf", lists, n_rows_padded, out_ids, out_scores);
   if (rc != CRAG_OK) return rc;
-  const SearchPlan sp = plan_search(k >= 1 && k <= 128 ? k : 1);
-  const IvfPlan ip = plan_ivf(sp, nlist, total_tiles);
+  const IvfPlan ip = plan_ivf(k >= 1 && k <= 128 ? k : 1, nlist, total_tiles, workspace);
   rc = check_scan_args("ivf", nq, k, 128, res, q, workspace, workspace_bytes, ip.total);
   if (rc != CRAG_OK) return rc;
-  return ivf_passes(res, q, IvfArgs{}, lists, k, k, nullptr, out_ids, out_scores, out_minmax, workspace, ip, sp,
+  return ivf_passes(res, q, IvfArgs{}, lists, k, k, nullptr, out_ids, out_scores, out_minmax, ip,
                     static_cast<cudaStream_t>(stream));
 }
 
@@ -591,7 +594,7 @@ extern "C" int crag_ivf_search_i8(const void* residuals_i8, const float* row_sca
   if (rc != CRAG_OK) return rc;
   if (nq < 1 || k < 1 || n_cand < k || n_cand > 128) return fail(CRAG_ERR_INVALID, "ivf_i8: need nq >= 1 and 1 <= k <= n_cand <= 128 (nq=%d k=%d n_cand=%d)", nq, k, n_cand);
   if (dim8 != (dim + 127) / 128 * 128) return fail(CRAG_ERR_INVALID, "ivf_i8: dim8 must be dim rounded up to a multiple of 128 (dim=%d dim8=%d)", dim, dim8);
-  const IvfI8Plan plan = plan_ivf_i8(nlist, total_tiles, n_cand);
+  const IvfI8Plan plan = plan_ivf_i8(nlist, total_tiles, n_cand, workspace);
   rc = check_scan_args("ivf_i8", nq, n_cand, 128, res, q, workspace, workspace_bytes, plan.total);
   if (rc == CRAG_OK) rc = check_operand("ivf_i8", rescore.rows);
   if (rc == CRAG_OK) rc = check_operand("ivf_i8", rescore.queries);
@@ -600,32 +603,32 @@ extern "C" int crag_ivf_search_i8(const void* residuals_i8, const float* row_sca
   // the bf16 residuals may be page-locked host memory: refused before any launch if pageable
   rc = device_readable(residuals_bf16, &rescore.rows.ptr, "ivf_i8");
   if (rc != CRAG_OK) return rc;
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  rescore.cand_ids = reinterpret_cast<int64_t*>(ws + plan.cand_ids_off);
-  rescore.cand_scores = reinterpret_cast<float*>(ws + plan.cand_scores_off);
-  return ivf_passes(res, q, I8IvfArgs{{}, {row_scales, query_scales}}, lists, n_cand, k, &rescore, out_ids, out_scores, out_minmax, workspace, plan.ivf,
-                    plan_search(n_cand), static_cast<cudaStream_t>(stream));
+  rescore.cand_ids = plan.cand_ids;
+  rescore.cand_scores = plan.cand_scores;
+  return ivf_passes(res, q, I8IvfArgs{{}, {row_scales, query_scales}}, lists, n_cand, k, &rescore, out_ids, out_scores, out_minmax, plan.ivf,
+                    static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int crag_search_scan(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,
                                 const void* queries, int nq, int k, void* workspace, size_t workspace_bytes,
                                 crag_stream_t stream) {
   const Operand c{corpus, n_rows, dim, corpus_row_stride, kBf16, "corpus"}, q{queries, nq, dim, dim, kBf16, "queries"};
-  const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1);
-  int rc = check_scan_args("search", nq, k, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
+  const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1, workspace);
+  int rc = check_scan_args("search", nq, k, 128, c, q, workspace, workspace_bytes, plan.parts_bytes);
   if (rc != CRAG_OK) return rc;
   if (nq > kNQ) return fail(CRAG_ERR_INVALID, "crag_search_scan handles one pass of at most %d queries (nq=%d)", kNQ, nq);
-  return scan_pass(c, q, k, nullptr, NoIvfArgs{}, workspace, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
+  return scan_pass(c, q, k, nullptr, NoIvfArgs{}, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int crag_search_finalize(const void* workspace, size_t workspace_bytes, int64_t n_rows, int nq, int k,
                                     int64_t row_offset, int64_t* out_ids, float* out_scores, float* out_minmax,
                                     crag_stream_t stream) {
   if (nq < 1 || nq > kNQ || k < 1 || k > 128) return fail(CRAG_ERR_INVALID, "crag_search_finalize: bad nq/k (nq=%d k=%d)", nq, k);
-  const SearchPlan plan = plan_search(k);
-  if (!workspace || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "crag_search_finalize: null pointer");
-  if (workspace_bytes < plan.keys_bytes + plan.minmax_bytes) return fail(CRAG_ERR_WORKSPACE, "crag_search_finalize: workspace too small");
-  return finalize_parts(workspace, scan_grid(n_rows, plan), nq, k, row_offset, out_ids, out_scores, out_minmax, nullptr, plan,
+  const SearchPlan plan = plan_search(k, workspace);
+  if (!out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "crag_search_finalize: null pointer");
+  const int rc = check_workspace("crag_search_finalize", workspace, workspace_bytes, plan.parts_bytes);
+  if (rc != CRAG_OK) return rc;
+  return finalize_parts(scan_grid(n_rows, plan), nq, k, row_offset, out_ids, out_scores, out_minmax, nullptr, plan,
                         static_cast<cudaStream_t>(stream));
 }
 
@@ -635,11 +638,11 @@ extern "C" int crag_search_topk_after(const void* corpus, int64_t n_rows, int di
                                       float* out_minmax, uint64_t* last_keys, void* workspace,
                                       size_t workspace_bytes, crag_stream_t stream) {
   const Operand c{corpus, n_rows, dim, corpus_row_stride, kBf16, "corpus"}, q{queries, nq, dim, dim, kBf16, "queries"};
-  const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1);
-  int rc = check_scan_args("search", nq, k, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
+  const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1, workspace);
+  int rc = check_scan_args("search", nq, k, 128, c, q, workspace, workspace_bytes, plan.parts_bytes);
   if (rc != CRAG_OK) return rc;
   if (!out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "search: null output pointer");
-  return topk_passes(c, q, k, row_offset, after_keys, NoIvfArgs{}, out_ids, out_scores, out_minmax, last_keys, workspace,
+  return topk_passes(c, q, k, row_offset, after_keys, NoIvfArgs{}, out_ids, out_scores, out_minmax, last_keys,
                      workspace_bytes, plan, static_cast<cudaStream_t>(stream));
 }
 
@@ -657,12 +660,12 @@ extern "C" int crag_search_topk_i8(const void* corpus_i8, const float* row_scale
                                    const float* query_scales, int nq, int k, int64_t* out_ids, float* out_scores,
                                    float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream) {
   const Operand c{corpus_i8, n_rows, dim8, row_stride, kS8, "corpus"}, q{queries_i8, nq, dim8, dim8, kS8, "queries"};
-  const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1);
-  int rc = check_scan_args("search_i8", nq, k, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
+  const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1, workspace);
+  int rc = check_scan_args("search_i8", nq, k, 128, c, q, workspace, workspace_bytes, plan.parts_bytes);
   if (rc != CRAG_OK) return rc;
   if (!query_scales || !out_ids || !out_scores || (n_rows > 0 && !row_scales)) return fail(CRAG_ERR_INVALID, "search_i8: null pointer");
   return topk_passes(c, q, k, row_offset, nullptr, I8Args{row_scales, query_scales}, out_ids, out_scores, out_minmax,
-                     nullptr, workspace, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
+                     nullptr, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------ exact top-k for large k / many queries
@@ -671,12 +674,22 @@ extern "C" int crag_search_topk_i8(const void* corpus_i8, const float* row_scale
 namespace crag {
 namespace {
 inline int64_t knn_ld(int64_t n_rows) { return ((n_rows > 0 ? n_rows : 1) + 3) & ~int64_t(3); }
+
+// Workspace of crag_knn_topk: the fp32 score block [q_chunk][knn_ld(n_rows)]
+struct KnnWorkspace { float* block; size_t total; };
+KnnWorkspace knn_workspace(int64_t n_rows, int q_chunk, void* ws = nullptr) {
+  WsCursor c(ws);
+  KnnWorkspace w;
+  w.block = c.take<float>(size_t(q_chunk) * size_t(knn_ld(n_rows)));
+  w.total = c.bytes;
+  return w;
+}
 }  // namespace
 }  // namespace crag
 
 extern "C" size_t crag_knn_workspace_bytes(int64_t n_rows, int q_chunk) {
   if (n_rows < 0 || q_chunk < 1) return 0;
-  return (size_t(q_chunk) * size_t(knn_ld(n_rows)) * 4 + 255) & ~size_t(255);
+  return knn_workspace(n_rows, q_chunk).total;
 }
 
 extern "C" int crag_knn_topk(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride, int64_t row_offset,
@@ -692,7 +705,7 @@ extern "C" int crag_knn_topk(const void* corpus, int64_t n_rows, int dim, int64_
   const size_t fit = workspace_bytes / per_query;
   if (fit < 1) return fail(CRAG_ERR_WORKSPACE, "knn: workspace %zu < %zu bytes (one query's score row)", workspace_bytes, per_query);
   const int q_chunk = fit < size_t(nq) ? int(fit) : nq;
-  float* block = static_cast<float*>(workspace);
+  float* block = knn_workspace(n_rows, q_chunk, workspace).block;
   for (int q0 = 0; q0 < nq; q0 += q_chunk) {
     const int nqc = (nq - q0) < q_chunk ? (nq - q0) : q_chunk;
     rc = gemm_scores_f32(static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, dim, corpus, corpus_row_stride,
@@ -765,8 +778,8 @@ __global__ void minmax_reduce_kernel(const float* __restrict__ part_minmax, int 
 // Score-all passes (the scan with ScoreArgs), one per block of 32 queries.  Block q0 stores its scores from row q0 of
 // sa.out on, or, in assignment mode (sa.best_id set), updates every row's running argmax with ids counted from q0.
 // out_minmax (may be null) receives each query's (min, max).
-int score_passes(const Operand& corpus, const Operand& queries, ScoreArgs sa, float* out_minmax, void* workspace,
-                 const SearchPlan& plan, cudaStream_t stream) {
+int score_passes(const Operand& corpus, const Operand& queries, ScoreArgs sa, float* out_minmax, const SearchPlan& plan,
+                 cudaStream_t stream) {
   const int nq = int(queries.rows);
   const int grid = scan_grid(corpus.rows, plan);
   if (grid == 0) {
@@ -776,7 +789,6 @@ int score_passes(const Operand& corpus, const Operand& queries, ScoreArgs sa, fl
     }
     return CRAG_OK;
   }
-  float* part_minmax = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + plan.keys_bytes);
   CUtensorMap tm_corpus;
   int rc = make_tmap(&tm_corpus, corpus, kTileRows);
   if (rc != CRAG_OK) return rc;
@@ -788,10 +800,10 @@ int score_passes(const Operand& corpus, const Operand& queries, ScoreArgs sa, fl
     ScoreArgs pass = sa;
     if (sa.best_id) pass.base_id = q0;
     else pass.out = sa.out + int64_t(q0) * sa.ld;
-    rc = launch_scan<16, 16, 7>(tm_corpus, tm_q, int(corpus.rows), corpus.num_kb(), nqc, 1, grid, nullptr, nullptr, 0u, 0, nullptr, part_minmax, pass, stream);
+    rc = launch_scan<16, 16, 7>(tm_corpus, tm_q, int(corpus.rows), corpus.num_kb(), nqc, 1, grid, nullptr, nullptr, 0u, 0, nullptr, plan.part_minmax, pass, stream);
     if (rc != CRAG_OK) return rc;
     if (out_minmax) {
-      minmax_reduce_kernel<<<nqc, 32, 0, stream>>>(part_minmax, grid, nqc, out_minmax + size_t(q0) * 2);
+      minmax_reduce_kernel<<<nqc, 32, 0, stream>>>(plan.part_minmax, grid, nqc, out_minmax + size_t(q0) * 2);
       CRAG_CUDA_OK(cudaGetLastError());
     }
   }
@@ -804,18 +816,18 @@ extern "C" int crag_search_scores(const void* corpus, int64_t n_rows, int dim, i
                                   const void* queries, int nq, float* out_scores, int64_t out_ld, float* out_minmax,
                                   void* workspace, size_t workspace_bytes, crag_stream_t stream) {
   const Operand c{corpus, n_rows, dim, corpus_row_stride, kBf16, "corpus"}, q{queries, nq, dim, dim, kBf16, "queries"};
-  const SearchPlan plan = plan_search(1);
-  int rc = check_scan_args("search", nq, 1, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
+  const SearchPlan plan = plan_search(1, workspace);
+  int rc = check_scan_args("search", nq, 1, 128, c, q, workspace, workspace_bytes, plan.parts_bytes);
   if (rc != CRAG_OK) return rc;
   if (!out_scores || out_ld < n_rows) return fail(CRAG_ERR_INVALID, "crag_search_scores: need out_scores and out_ld >= n_rows");
-  return score_passes(c, q, ScoreArgs{out_scores, out_ld, nullptr, nullptr, 0}, out_minmax, workspace, plan,
+  return score_passes(c, q, ScoreArgs{out_scores, out_ld, nullptr, nullptr, 0}, out_minmax, plan,
                       static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------ fused finalize + exchange (row-sharded index)
 extern "C" size_t crag_exchange_buffer_bytes(int world) {
   if (world < 1 || world > kXMaxWorld) return 0;
-  return (xchg_total_bytes(world) + 255) & ~size_t(255);
+  return ws_round(xchg_total_bytes(world));
 }
 
 extern "C" int crag_search_finalize_exchange(const void* workspace, size_t workspace_bytes, int64_t n_rows, int nq, int k,
@@ -825,15 +837,14 @@ extern "C" int crag_search_finalize_exchange(const void* workspace, size_t works
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (nq < 1 || nq > kNQ || k < 1 || k > 128) return fail(CRAG_ERR_INVALID, "crag_search_finalize_exchange: bad nq/k (nq=%d k=%d)", nq, k);
   if (world < 1 || world > kXMaxWorld || rank < 0 || rank >= world) return fail(CRAG_ERR_INVALID, "crag_search_finalize_exchange: bad rank/world (%d/%d)", rank, world);
-  if (!workspace || !peer_bufs || !epochs || !status || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "crag_search_finalize_exchange: null pointer");
-  const SearchPlan plan = plan_search(k);
-  if (workspace_bytes < plan.keys_bytes + plan.minmax_bytes) return fail(CRAG_ERR_WORKSPACE, "crag_search_finalize_exchange: workspace too small");
-  const uint64_t* part_keys = static_cast<const uint64_t*>(workspace);
-  const float* part_minmax = reinterpret_cast<const float*>(static_cast<const uint8_t*>(workspace) + plan.keys_bytes);
+  if (!peer_bufs || !epochs || !status || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "crag_search_finalize_exchange: null pointer");
+  const SearchPlan plan = plan_search(k, workspace);
+  const int rc = check_workspace("crag_search_finalize_exchange", workspace, workspace_bytes, plan.parts_bytes);
+  if (rc != CRAG_OK) return rc;
   const int parts = scan_grid(n_rows, plan);
   with_merge_tier(k, [&](auto tier) {   // one CTA per query
     constexpr int T = decltype(tier)::value;
-    finalize_exchange_kernel<T, T><<<nq, 128, 0, stream>>>(part_keys, part_minmax, parts, nq, k, row_offset, peer_bufs, rank,
+    finalize_exchange_kernel<T, T><<<nq, 128, 0, stream>>>(plan.part_keys, plan.part_minmax, parts, nq, k, row_offset, peer_bufs, rank,
                                                            world, epochs, status, out_ids, out_scores, out_minmax);
   });
   CRAG_CUDA_OK(cudaGetLastError());
@@ -848,11 +859,11 @@ extern "C" int crag_ivf_assign(const void* rows, int64_t n_rows, int dim, int64_
                                int nlist, float* best_score, int32_t* best_id, void* workspace, size_t workspace_bytes,
                                crag_stream_t stream) {
   const Operand c{rows, n_rows, dim, row_stride, kBf16, "rows"}, q{centroids, nlist, dim, dim, kBf16, "centroids"};
-  const SearchPlan plan = plan_search(1);
-  int rc = check_scan_args("search", nlist, 1, 128, c, q, workspace, workspace_bytes, plan.keys_bytes + plan.minmax_bytes);
+  const SearchPlan plan = plan_search(1, workspace);
+  int rc = check_scan_args("search", nlist, 1, 128, c, q, workspace, workspace_bytes, plan.parts_bytes);
   if (rc != CRAG_OK) return rc;
   if (!best_score || !best_id) return fail(CRAG_ERR_INVALID, "crag_ivf_assign: null output pointer");
   // the pass over centroid block 0 initialises every row's running best (-inf, list 0); later passes update it
-  return score_passes(c, q, ScoreArgs{nullptr, 0, best_score, best_id, 0}, nullptr, workspace, plan,
+  return score_passes(c, q, ScoreArgs{nullptr, 0, best_score, best_id, 0}, nullptr, plan,
                       static_cast<cudaStream_t>(stream));
 }

@@ -23,6 +23,8 @@
 #include <stdint.h>
 #include <cuda_runtime.h>
 
+#include "workspace.cuh"
+
 #ifndef CRAG_EMULATED_PTX
 #define CRAG_DYNAMIC_SHARED(type, name) extern __shared__ type name[]
 #endif
@@ -66,40 +68,54 @@ __host__ __device__ inline int umap_p(int64_t n, int d) {
   return int(n < p ? n : p);
 }
 
+// Workspace of the fuzzy graph: the rows' distance sums [n] and their mean (fp64).
+struct UmapFuzzyWorkspace { double *rowsum, *mean; size_t total; };
+inline UmapFuzzyWorkspace umap_fuzzy_workspace(int64_t n, void* ws = nullptr) {
+  WsCursor c(ws);
+  UmapFuzzyWorkspace w;
+  w.rowsum = c.take<double>(size_t(n));
+  w.mean = c.take<double>(1);
+  w.total = c.bytes;
+  return w;
+}
+
+// The spectral start.  Workspace `ws`: degrees and D^-1/2 [n], V and W [n][p], Gram partials [chunks][p][p], R^-1
+// [p][p], eigenvectors + eigenvalues [p][p] + [p], Ritz vectors [n][d] (fp64 throughout).
 struct UmapSpectralPlan {
   int p, chunks;
   int64_t chunk_rows;
-  size_t deg_off, dis_off, v_off, w_off, part_off, rinv_off, q_off, yr_off, total;
+  double *deg, *dis, *v, *w, *part, *rinv, *q, *yr;   // the workspace's regions (null when only sized)
+  size_t total;                                        // workspace bytes
 };
-
-inline size_t umap_align(size_t b) { return (b + 255) & ~size_t(255); }
-
-inline size_t umap_fuzzy_ws(int64_t n) { return umap_align(sizeof(double) * size_t(n)) + umap_align(sizeof(double)); }
-
-// Workspace of the spectral start: degrees and D^-1/2 [n], V and W [n][p], Gram partials [chunks][p][p], R^-1 [p][p],
-// eigenvectors + eigenvalues [p][p] + [p], Ritz vectors [n][d] (fp64 throughout).
-inline UmapSpectralPlan plan_umap_spectral(int64_t n, int d) {
+inline UmapSpectralPlan plan_umap_spectral(int64_t n, int d, void* ws = nullptr) {
   UmapSpectralPlan s;
   s.p = umap_p(n, d);
   const int64_t want = (n + kUmapChunkRows - 1) / kUmapChunkRows;
   s.chunks = int(want < 1 ? 1 : want > kUmapMaxChunks ? kUmapMaxChunks : want);
   s.chunk_rows = (n + s.chunks - 1) / s.chunks;
   const size_t P = size_t(s.p), N = size_t(n);
-  size_t o = 0;
-  s.deg_off = o;  o += umap_align(sizeof(double) * N);
-  s.dis_off = o;  o += umap_align(sizeof(double) * N);
-  s.v_off = o;    o += umap_align(sizeof(double) * N * P);
-  s.w_off = o;    o += umap_align(sizeof(double) * N * P);
-  s.part_off = o; o += umap_align(sizeof(double) * size_t(s.chunks) * P * P);
-  s.rinv_off = o; o += umap_align(sizeof(double) * P * P);
-  s.q_off = o;    o += umap_align(sizeof(double) * (P * P + P));
-  s.yr_off = o;   o += umap_align(sizeof(double) * N * size_t(d));
-  s.total = o;
+  WsCursor c(ws);
+  s.deg = c.take<double>(N);
+  s.dis = c.take<double>(N);
+  s.v = c.take<double>(N * P);
+  s.w = c.take<double>(N * P);
+  s.part = c.take<double>(size_t(s.chunks) * P * P);
+  s.rinv = c.take<double>(P * P);
+  s.q = c.take<double>(P * P + P);
+  s.yr = c.take<double>(N * size_t(d));
+  s.total = c.bytes;
   return s;
 }
 
-// the second layout buffer [n][d]
-inline size_t umap_optimize_ws(int64_t n, int d) { return umap_align(sizeof(float) * size_t(n) * size_t(d)); }
+// Workspace of the layout: the second layout buffer [n][d].
+struct UmapOptimizeWorkspace { float* other; size_t total; };
+inline UmapOptimizeWorkspace umap_optimize_workspace(int64_t n, int d, void* ws = nullptr) {
+  WsCursor c(ws);
+  UmapOptimizeWorkspace w;
+  w.other = c.take<float>(size_t(n) * size_t(d));
+  w.total = c.bytes;
+  return w;
+}
 
 // The schedule counters advance as umap-learn's do, a product then a sum, never contracted into one fma.
 #ifdef CRAG_EMULATED_PTX

@@ -49,6 +49,17 @@ def test_search_argument_validation(lib, p):
     assert call(ids=None) == INVALID
 
 
+def test_finalize_workspace_validation(lib, p):
+    """The finalize entries read 8-byte keys from the scan's workspace: a misaligned one is refused before a launch."""
+    fin = lambda ws=p, wsb=1 << 24: lib.crag_search_finalize(ws, wsb, 100, 4, 10, 0, p, p, p, None)
+    xchg = lambda ws=p, wsb=1 << 24: lib.crag_search_finalize_exchange(ws, wsb, 100, 4, 10, 0, p, 0, 2, p, p, p, p, p,
+                                                                       None)
+    for call in (fin, xchg):
+        assert call(ws=None) == INVALID and "null" in err(lib)
+        assert call(ws=p + 8) == INVALID and "256-byte aligned" in err(lib)
+        assert call(wsb=16) == WORKSPACE and "workspace 16 <" in err(lib)
+
+
 def test_merge_gemm_and_encoder_piece_validation(lib, p):
     assert lib.crag_merge_topk(p, p, None, 2, 0, 10, p, p, None, None) == INVALID
     assert lib.crag_merge_topk(p, p, None, 2, 4, 200, p, p, None, None) == INVALID

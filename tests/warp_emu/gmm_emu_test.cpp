@@ -70,22 +70,8 @@ struct Out {
 static Out run(const Case& c, uint64_t seed) {
   const int64_t n = c.n;
   const int d = c.d, M = c.M;
-  const GmmPlan p = plan_gmm(n, d, M);
-  std::vector<uint8_t> ws_mem(p.total + 256, 0xFF);          // NaN everywhere: nothing may read what it did not write
-  uint8_t* ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws_mem.data()) + 255) & ~uintptr_t(255));
-  double* glob = reinterpret_cast<double*>(ws + p.glob_off);
-  GmmState* state = reinterpret_cast<GmmState*>(ws + p.state_off);
-  double* xc = reinterpret_cast<double*>(ws + p.xc_off);
-  double* dist = reinterpret_cast<double*>(ws + p.dist_off);
-  double* centres = reinterpret_cast<double*>(ws + p.centre_off);
-  double* lsum = reinterpret_cast<double*>(ws + p.lsum_off);
-  int32_t* lchg = reinterpret_cast<int32_t*>(ws + p.lchg_off);
-  double* mu = reinterpret_cast<double*>(ws + p.mu_off);
-  double* prec = reinterpret_cast<double*>(ws + p.prec_off);
-  double* cst = reinterpret_cast<double*>(ws + p.cst_off);
-  double* wt = reinterpret_cast<double*>(ws + p.wt_off);
-  double* esum = reinterpret_cast<double*>(ws + p.esum_off);
-  double* lse = reinterpret_cast<double*>(ws + p.lse_off);
+  warp_emu::Workspace ws(plan_gmm(n, d, M).total, kWsAlign, 0xFF);   // NaN everywhere
+  const GmmPlan p = plan_gmm(n, d, M, ws.base);
   const int R = p.chunks, C = p.components;
   const unsigned grid = unsigned(R * M);
   Out o;
@@ -105,49 +91,49 @@ static Out run(const Case& c, uint64_t seed) {
   uint64_t s = seed;
   auto next = [&]() { return seed ? ++s : 0; };
 
-  launch(next(), 1, 1024, sizeof(double) * 1024, [&] { gmm_moments_kernel(x, n, d, M, glob, state); });
-  launch(next(), 4, kGmmThreads, 0, [&] { gmm_centre_kernel(x, n, d, M, glob, xc, labels); });
+  launch(next(), 1, 1024, sizeof(double) * 1024, [&] { gmm_moments_kernel(x, n, d, M, p.glob, p.state); });
+  launch(next(), 4, kGmmThreads, 0, [&] { gmm_centre_kernel(x, n, d, M, p.glob, p.xc, labels); });
   launch(next(), M, kGmmSeedThreads, seed_smem,
-         [&] { gmm_seed_kernel(xc, n, d, c.first.data(), c.draws.data(), dist, centres, o.seeds.data()); });
+         [&] { gmm_seed_kernel(p.xc, n, d, c.first.data(), c.draws.data(), p.dist, p.centres, o.seeds.data()); });
   for (int it = 0; it < kGmmLloydIters; ++it) {
     launch(next(), grid, kGmmThreads, assign_smem, [&] {
-      gmm_lloyd_assign_kernel(xc, n, d, M, R, p.chunk_rows, 1, state, centres, labels, dist, lsum, lchg);
+      gmm_lloyd_assign_kernel(p.xc, n, d, M, R, p.chunk_rows, 1, p.state, p.centres, labels, p.dist, p.lsum, p.lchg);
     });
     launch(next(), M, kGmmThreads, update_smem, [&] {
-      gmm_lloyd_update_kernel(xc, n, d, M, R, it, glob, state, centres, labels, dist, lsum, lchg);
+      gmm_lloyd_update_kernel(p.xc, n, d, M, R, it, p.glob, p.state, p.centres, labels, p.dist, p.lsum, p.lchg);
     });
   }
   launch(next(), grid, kGmmThreads, assign_smem, [&] {
-    gmm_lloyd_assign_kernel(xc, n, d, M, R, p.chunk_rows, 0, state, centres, labels, dist, lsum, lchg);
+    gmm_lloyd_assign_kernel(p.xc, n, d, M, R, p.chunk_rows, 0, p.state, p.centres, labels, p.dist, p.lsum, p.lchg);
   });
   launch(next(), unsigned((C * d + kGmmThreads - 1) / kGmmThreads), kGmmThreads, 0,
-         [&] { gmm_em_setup_kernel(d, C, glob, centres, mu); });
+         [&] { gmm_em_setup_kernel(d, C, p.glob, p.centres, p.mu); });
   launch(next(), grid, kGmmThreads, stats_smem, [&] {
-    gmm_em_stats_kernel(x, n, d, M, R, p.chunk_rows, kGmmInit, state, nullptr, labels, mu, prec, cst, esum, lse, nullptr);
+    gmm_em_stats_kernel(x, n, d, M, R, p.chunk_rows, kGmmInit, p.state, nullptr, labels, p.mu, p.prec, p.cst, p.esum, p.lse, nullptr);
   });
   launch(next(), M, kGmmThreads, m_smem,
-         [&] { gmm_mstep_kernel(n, d, M, R, kGmmInit, 0, state, mu, prec, cst, wt, esum, lse); });
+         [&] { gmm_mstep_kernel(n, d, M, R, kGmmInit, 0, p.state, p.mu, p.prec, p.cst, p.wt, p.esum, p.lse); });
   for (int it = 1; it <= kGmmEmIters; ++it) {
     launch(next(), grid, kGmmThreads, stats_smem, [&] {
-      gmm_em_stats_kernel(x, n, d, M, R, p.chunk_rows, kGmmStep, state, nullptr, labels, mu, prec, cst, esum, lse,
+      gmm_em_stats_kernel(x, n, d, M, R, p.chunk_rows, kGmmStep, p.state, nullptr, labels, p.mu, p.prec, p.cst, p.esum, p.lse,
                           nullptr);
     });
     launch(next(), M, kGmmThreads, m_smem,
-           [&] { gmm_mstep_kernel(n, d, M, R, kGmmStep, it, state, mu, prec, cst, wt, esum, lse); });
+           [&] { gmm_mstep_kernel(n, d, M, R, kGmmStep, it, p.state, p.mu, p.prec, p.cst, p.wt, p.esum, p.lse); });
   }
   launch(next(), grid, kGmmThreads, stats_smem, [&] {
-    gmm_em_stats_kernel(x, n, d, M, R, p.chunk_rows, kGmmScore, state, nullptr, labels, mu, prec, cst, esum, lse, nullptr);
+    gmm_em_stats_kernel(x, n, d, M, R, p.chunk_rows, kGmmScore, p.state, nullptr, labels, p.mu, p.prec, p.cst, p.esum, p.lse, nullptr);
   });
   launch(next(), 1, kGmmMaxM, sizeof(double) * (kGmmMaxM + 1), [&] {
-    gmm_select_kernel(n, d, M, R, state, mu, wt, lse, o.bic.data(), o.iters.data(), o.conv.data(), o.best.data(),
+    gmm_select_kernel(n, d, M, R, p.state, p.mu, p.wt, p.lse, o.bic.data(), o.iters.data(), o.conv.data(), o.best.data(),
                       o.weights.data(), o.means.data());
   });
   launch(next(), unsigned(R), kGmmThreads, stats_smem, [&] {
-    gmm_em_stats_kernel(x, n, d, M, R, p.chunk_rows, kGmmResp, state, o.best.data(), labels, mu, prec, cst, esum, lse,
+    gmm_em_stats_kernel(x, n, d, M, R, p.chunk_rows, kGmmResp, p.state, o.best.data(), labels, p.mu, p.prec, p.cst, p.esum, p.lse,
                         o.memb.data());
   });
   o.memb.resize(size_t(n) * o.best[0]);
-  for (int m = 0; m < M; ++m) o.lloyd_iters.push_back(state[m].lloyd_iters);
+  for (int m = 0; m < M; ++m) o.lloyd_iters.push_back(p.state[m].lloyd_iters);
   return o;
 }
 
@@ -165,43 +151,34 @@ static void run_lloyd(const char* in, const char* out, uint64_t seed) {
   read_into(f, c0, int64_t(m) * d);
   fclose(f);
   const int M = m;
-  const GmmPlan p = plan_gmm(n, d, M);
-  std::vector<uint8_t> ws_mem(p.total + 256, 0xFF);
-  uint8_t* ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws_mem.data()) + 255) & ~uintptr_t(255));
-  double* glob = reinterpret_cast<double*>(ws + p.glob_off);
-  GmmState* state = reinterpret_cast<GmmState*>(ws + p.state_off);
-  double* xc = reinterpret_cast<double*>(ws + p.xc_off);
-  int32_t* labels = reinterpret_cast<int32_t*>(ws + p.labels_off);
-  double* dist = reinterpret_cast<double*>(ws + p.dist_off);
-  double* centres = reinterpret_cast<double*>(ws + p.centre_off);
-  double* lsum = reinterpret_cast<double*>(ws + p.lsum_off);
-  int32_t* lchg = reinterpret_cast<int32_t*>(ws + p.lchg_off);
+  warp_emu::Workspace ws(plan_gmm(n, d, M).total, kWsAlign, 0xFF);
+  const GmmPlan p = plan_gmm(n, d, M, ws.base);
   const int R = p.chunks;
   const size_t assign_smem = sizeof(double) * size_t(M * d + kGmmThreads * d) + sizeof(int32_t) * 2 * kGmmThreads;
   const size_t update_smem = sizeof(double) * size_t(M * (d + 1) + kGmmThreads) +
                              sizeof(int64_t) * (kGmmMaxM + kGmmThreads) + sizeof(int) * (kGmmMaxM + 1);
   uint64_t s = seed;
   auto next = [&]() { return seed ? ++s : 0; };
-  launch(next(), 1, 1024, sizeof(double) * 1024, [&] { gmm_moments_kernel(x.data(), n, d, M, glob, state); });
-  launch(next(), 4, kGmmThreads, 0, [&] { gmm_centre_kernel(x.data(), n, d, M, glob, xc, labels); });
-  for (int k = 0; k + 1 < M; ++k) state[k].lloyd_done = state[k].lloyd_strict = 1;
-  memcpy(centres + int64_t(gmm_comp_off(m)) * d, c0.data(), c0.size() * sizeof(double));
+  launch(next(), 1, 1024, sizeof(double) * 1024, [&] { gmm_moments_kernel(x.data(), n, d, M, p.glob, p.state); });
+  launch(next(), 4, kGmmThreads, 0, [&] { gmm_centre_kernel(x.data(), n, d, M, p.glob, p.xc, p.labels); });
+  for (int k = 0; k + 1 < M; ++k) p.state[k].lloyd_done = p.state[k].lloyd_strict = 1;
+  memcpy(p.centres + int64_t(gmm_comp_off(m)) * d, c0.data(), c0.size() * sizeof(double));
   for (int it = 0; it < kGmmLloydIters; ++it) {
     launch(next(), unsigned(R * M), kGmmThreads, assign_smem, [&] {
-      gmm_lloyd_assign_kernel(xc, n, d, M, R, p.chunk_rows, 1, state, centres, labels, dist, lsum, lchg);
+      gmm_lloyd_assign_kernel(p.xc, n, d, M, R, p.chunk_rows, 1, p.state, p.centres, p.labels, p.dist, p.lsum, p.lchg);
     });
     launch(next(), M, kGmmThreads, update_smem, [&] {
-      gmm_lloyd_update_kernel(xc, n, d, M, R, it, glob, state, centres, labels, dist, lsum, lchg);
+      gmm_lloyd_update_kernel(p.xc, n, d, M, R, it, p.glob, p.state, p.centres, p.labels, p.dist, p.lsum, p.lchg);
     });
   }
   launch(next(), unsigned(R * M), kGmmThreads, assign_smem, [&] {
-    gmm_lloyd_assign_kernel(xc, n, d, M, R, p.chunk_rows, 0, state, centres, labels, dist, lsum, lchg);
+    gmm_lloyd_assign_kernel(p.xc, n, d, M, R, p.chunk_rows, 0, p.state, p.centres, p.labels, p.dist, p.lsum, p.lchg);
   });
   FILE* o = fopen(out, "wb");
   REQUIRE(o != nullptr, "cannot write %s", out);
-  REQUIRE(fwrite(labels + int64_t(m - 1) * n, 4, size_t(n), o) == size_t(n), "short write");
-  REQUIRE(fwrite(&state[m - 1].lloyd_iters, 4, 1, o) == 1, "short write");
-  REQUIRE(fwrite(centres + int64_t(gmm_comp_off(m)) * d, 8, c0.size(), o) == c0.size(), "short write");
+  REQUIRE(fwrite(p.labels + int64_t(m - 1) * n, 4, size_t(n), o) == size_t(n), "short write");
+  REQUIRE(fwrite(&p.state[m - 1].lloyd_iters, 4, 1, o) == 1, "short write");
+  REQUIRE(fwrite(p.centres + int64_t(gmm_comp_off(m)) * d, 8, c0.size(), o) == c0.size(), "short write");
   fclose(o);
 }
 

@@ -49,22 +49,19 @@ static void test_rank(int64_t n, int levels, bool specials) {
     scores[0] = 0.0f; scores[1] = -0.0f; scores[2] = INFINITY; scores[3] = -INFINITY;
     scores[4] = 1e-42f; scores[5] = -1e-42f; scores[6] = scores[7];
   }
-  const SortPlan p = plan_sort(n);
-  std::vector<uint8_t> ws(p.total + 256, 0xAB);
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws.data()) + 255) & ~uintptr_t(255));
-  uint32_t* keys[2] = {reinterpret_cast<uint32_t*>(base), reinterpret_cast<uint32_t*>(base + p.key_bytes)};
-  uint32_t* vals[2] = {reinterpret_cast<uint32_t*>(base + 2 * p.key_bytes), reinterpret_cast<uint32_t*>(base + 2 * p.key_bytes + p.val_bytes)};
-  uint32_t* hist = reinterpret_cast<uint32_t*>(base + 2 * p.key_bytes + 2 * p.val_bytes);
+  warp_emu::Workspace ws(plan_sort(n).total, kWsAlign, 0xAB);
+  const SortPlan p = plan_sort(n, ws.base);
+  uint32_t* hist = p.hist;
   uint32_t* totals = hist + size_t(256) * p.n_warps;
   std::vector<int64_t> out_ids(n, -7);
   std::vector<float> out_scores(n, -7.f);
   const float* sc = scores.data();
   for (int pass = 0; pass < 4; ++pass) {          // the launch sequence of crag_rank_scores (rank_all.cu)
     const int shift = pass * 8;
-    const uint32_t* kin = pass ? keys[(pass - 1) & 1] : nullptr;
-    const uint32_t* vin = pass ? vals[(pass - 1) & 1] : nullptr;
-    uint32_t* kout = keys[pass & 1];
-    uint32_t* vout = vals[pass & 1];
+    const uint32_t* kin = pass ? p.keys[(pass - 1) & 1] : nullptr;
+    const uint32_t* vin = pass ? p.vals[(pass - 1) & 1] : nullptr;
+    uint32_t* kout = p.keys[pass & 1];
+    uint32_t* vout = p.vals[pass & 1];
     memset(totals, 0, 256 * 4);
     if (pass == 0) warp_emu::launch(p.grid, kSortThreads, [&] { hist_kernel<true>(sc, nullptr, n, p.run, p.n_warps, shift, hist, totals); });
     else warp_emu::launch(p.grid, kSortThreads, [&] { hist_kernel<false>(nullptr, kin, n, p.run, p.n_warps, shift, hist, totals); });

@@ -68,29 +68,13 @@ static void launch(uint64_t seed, unsigned grid, int block, size_t smem, const s
 
 static unsigned blocks(int64_t items, int per_block) { return unsigned((items + per_block - 1) / per_block); }
 
-// aligned workspace filled with NaN bytes: nothing may read what it did not write
-struct Workspace {
-  std::vector<uint8_t> mem;
-  uint8_t* base;
-  explicit Workspace(size_t bytes) : mem(bytes + 256, 0xFF) {
-    base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(mem.data()) + 255) & ~uintptr_t(255));
-  }
-};
-
 // crag_ppr's sequence for reset b
 static std::vector<float> run_single(const Case& c, int64_t b) {
   const int64_t n = c.n, nnz = c.nnz;
   const int64_t n_out = c.n_out < 0 ? n : c.n_out;
   const int32_t* out_vertices = c.n_out < 0 ? nullptr : c.out_vertices.data();
-  const PprPlan p = plan_ppr(n, nnz);
-  Workspace w(p.total);
-  uint8_t* ws = w.base;
-  float* y[2] = {reinterpret_cast<float*>(ws), reinterpret_cast<float*>(ws + p.y_bytes)};
-  int32_t* seg_row = reinterpret_cast<int32_t*>(ws + p.seg_row_off);
-  int32_t* head_row = reinterpret_cast<int32_t*>(ws + p.head_row_off);
-  float* head_val = reinterpret_cast<float*>(ws + p.head_val_off);
-  float* carry = reinterpret_cast<float*>(ws + p.carry_off);
-  float* partials = reinterpret_cast<float*>(ws + p.partial_off);
+  warp_emu::Workspace ws(plan_ppr(n, nnz).total, kWsAlign, 0xFF);   // NaN everywhere
+  const PprPlan p = plan_ppr(n, nnz, ws.base);
   const int64_t* row_ptr = c.row_ptr.data();
   const int32_t* col = c.col.data();
   const float* coef = c.coef.data();
@@ -99,22 +83,22 @@ static std::vector<float> run_single(const Case& c, int64_t b) {
   std::vector<float> out(size_t(n_out), -7.f);
   if (c.iterations > 0)
     launch(0, blocks(p.segments + 1, kPprThreads), kPprThreads, 0,
-           [&] { ppr_plan_kernel(row_ptr, n, nnz, p.segments, seg_row, head_row); });
-  launch(0, blocks(n, kPprThreads), kPprThreads, 0, [&] { ppr_init_kernel(reset, d, n, y[0]); });
+           [&] { ppr_plan_kernel(row_ptr, n, nnz, p.segments, p.seg_row, p.head_row); });
+  launch(0, blocks(n, kPprThreads), kPprThreads, 0, [&] { ppr_init_kernel(reset, d, n, p.y[0]); });
   for (int64_t t = 0; t < c.iterations; ++t) {
-    const float* y_in = y[t & 1];
-    float* y_out = y[(t + 1) & 1];
+    const float* y_in = p.y[t & 1];
+    float* y_out = p.y[(t + 1) & 1];
     launch(0, blocks(p.segments, kPprStepWarps), kPprStepThreads, kPprStepSmemBytes, [&] {
-      ppr_step_kernel(row_ptr, col, coef, reset, d, y_in, y_out, seg_row, head_row, n, nnz, p.segments, head_val, carry);
+      ppr_step_kernel(row_ptr, col, coef, reset, d, y_in, y_out, p.seg_row, p.head_row, n, nnz, p.segments, p.head_val, p.carry);
     });
     launch(0, blocks(p.segments, kPprThreads), kPprThreads, 0,
-           [&] { ppr_fixup_kernel(row_ptr, reset, d, head_row, head_val, carry, p.segments, y_out); });
+           [&] { ppr_fixup_kernel(row_ptr, reset, d, p.head_row, p.head_val, p.carry, p.segments, y_out); });
   }
-  const float* y_T = y[c.iterations & 1];
-  launch(0, unsigned(p.sum_blocks), kPprThreads, kPprSumSmemBytes, [&] { ppr_sum_kernel(y_T, n, partials); });
+  const float* y_T = p.y[c.iterations & 1];
+  launch(0, unsigned(p.sum_blocks), kPprThreads, kPprSumSmemBytes, [&] { ppr_sum_kernel(y_T, n, p.partials); });
   if (n_out > 0)
     launch(0, blocks(n_out, kPprThreads), kPprThreads, kPprSumSmemBytes,
-           [&] { ppr_gather_kernel(y_T, partials, p.sum_blocks, out_vertices, n_out, out.data()); });
+           [&] { ppr_gather_kernel(y_T, p.partials, p.sum_blocks, out_vertices, n_out, out.data()); });
   return out;
 }
 
@@ -124,18 +108,9 @@ static std::vector<float> run_batch(const Case& c, int batch, uint64_t seed) {
   const int64_t n = c.n, nnz = c.nnz;
   const int64_t n_out = c.n_out < 0 ? n : c.n_out;
   const int32_t* out_vertices = c.n_out < 0 ? nullptr : c.out_vertices.data();
-  const PprBatchPlan p = plan_ppr_batch(n, nnz, batch);
+  warp_emu::Workspace ws(plan_ppr_batch(n, nnz, batch).total, kWsAlign, 0xFF);
+  const PprBatchPlan p = plan_ppr_batch(n, nnz, batch, ws.base);
   REQUIRE(p.width == W, "width %d for batch %d", p.width, batch);
-  Workspace w(p.total);
-  uint8_t* ws = w.base;
-  float* y[2] = {reinterpret_cast<float*>(ws), reinterpret_cast<float*>(ws + p.y_bytes)};
-  float* v = reinterpret_cast<float*>(ws + p.v_off);
-  int32_t* seg_row = reinterpret_cast<int32_t*>(ws + p.seg_row_off);
-  int32_t* head_row = reinterpret_cast<int32_t*>(ws + p.head_row_off);
-  float* head_val = reinterpret_cast<float*>(ws + p.head_val_off);
-  float* carry = reinterpret_cast<float*>(ws + p.carry_off);
-  float* partials = reinterpret_cast<float*>(ws + p.partial_off);
-  float* totals = reinterpret_cast<float*>(ws + p.total_off);
   const int64_t* row_ptr = c.row_ptr.data();
   const int32_t* col = c.col.data();
   const float* coef = c.coef.data();
@@ -144,27 +119,27 @@ static std::vector<float> run_batch(const Case& c, int batch, uint64_t seed) {
   std::vector<float> out(size_t(batch * n_out), -7.f);
   if (c.iterations > 0)
     launch(seed, blocks(p.segments + 1, kPprThreads), kPprThreads, 0,
-           [&] { ppr_plan_kernel(row_ptr, n, nnz, p.segments, seg_row, head_row); });
+           [&] { ppr_plan_kernel(row_ptr, n, nnz, p.segments, p.seg_row, p.head_row); });
   launch(seed, blocks(n * W, kPprThreads), kPprThreads, 0,
-         [&] { ppr_batch_init_kernel<W>(resets, batch, d, n, v, y[0]); });
+         [&] { ppr_batch_init_kernel<W>(resets, batch, d, n, p.v, p.y[0]); });
   for (int64_t t = 0; t < c.iterations; ++t) {
-    const float* y_in = y[t & 1];
-    float* y_out = y[(t + 1) & 1];
+    const float* y_in = p.y[t & 1];
+    float* y_out = p.y[(t + 1) & 1];
     launch(seed ? seed + 2 * t : 0, blocks(p.segments, kPprStepWarps), kPprStepThreads, kPprBatchStepSmemBytes, [&] {
-      ppr_batch_step_kernel<W>(row_ptr, col, coef, v, d, y_in, y_out, seg_row, head_row, n, nnz, p.segments, head_val,
-                               carry);
+      ppr_batch_step_kernel<W>(row_ptr, col, coef, p.v, d, y_in, y_out, p.seg_row, p.head_row, n, nnz, p.segments, p.head_val,
+                               p.carry);
     });
     launch(seed ? seed + 2 * t + 1 : 0, blocks(p.segments * W, kPprThreads), kPprThreads, 0,
-           [&] { ppr_batch_fixup_kernel<W>(row_ptr, v, d, head_row, head_val, carry, p.segments, y_out); });
+           [&] { ppr_batch_fixup_kernel<W>(row_ptr, p.v, d, p.head_row, p.head_val, p.carry, p.segments, y_out); });
   }
-  const float* y_T = y[c.iterations & 1];
-  launch(seed, unsigned(p.sum_blocks), kPprThreads, kPprSumSmemBytes, [&] { ppr_batch_sum_kernel<W>(y_T, n, partials); });
+  const float* y_T = p.y[c.iterations & 1];
+  launch(seed, unsigned(p.sum_blocks), kPprThreads, kPprSumSmemBytes, [&] { ppr_batch_sum_kernel<W>(y_T, n, p.partials); });
   launch(seed, unsigned(W), kPprThreads, kPprSumSmemBytes,
-         [&] { ppr_batch_total_kernel<W>(partials, p.sum_blocks, totals); });
+         [&] { ppr_batch_total_kernel<W>(p.partials, p.sum_blocks, p.totals); });
   const int64_t per_column = blocks(n_out, kPprThreads);
   if (n_out > 0)
     launch(seed, unsigned(per_column * batch), kPprThreads, 0,
-           [&] { ppr_batch_gather_kernel<W>(y_T, totals, out_vertices, n_out, per_column, out.data()); });
+           [&] { ppr_batch_gather_kernel<W>(y_T, p.totals, out_vertices, n_out, per_column, out.data()); });
   return out;
 }
 

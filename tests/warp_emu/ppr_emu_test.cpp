@@ -72,15 +72,8 @@ static std::vector<float> run(const Case& c, uint64_t seed) {
   const int64_t n = c.n, nnz = c.nnz;
   const int64_t n_out = c.n_out < 0 ? n : c.n_out;
   const int32_t* out_vertices = c.n_out < 0 ? nullptr : c.out_vertices.data();
-  const PprPlan p = plan_ppr(n, nnz);
-  std::vector<uint8_t> ws_mem(p.total + 256, 0xFF);          // NaN everywhere: nothing may read what it did not write
-  uint8_t* ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws_mem.data()) + 255) & ~uintptr_t(255));
-  float* y[2] = {reinterpret_cast<float*>(ws), reinterpret_cast<float*>(ws + p.y_bytes)};
-  int32_t* seg_row = reinterpret_cast<int32_t*>(ws + p.seg_row_off);
-  int32_t* head_row = reinterpret_cast<int32_t*>(ws + p.head_row_off);
-  float* head_val = reinterpret_cast<float*>(ws + p.head_val_off);
-  float* carry = reinterpret_cast<float*>(ws + p.carry_off);
-  float* partials = reinterpret_cast<float*>(ws + p.partial_off);
+  warp_emu::Workspace ws(plan_ppr(n, nnz).total, kWsAlign, 0xFF);   // NaN everywhere
+  const PprPlan p = plan_ppr(n, nnz, ws.base);
   const int64_t* row_ptr = c.row_ptr.data();
   const int32_t* col = c.col.data();
   const float* coef = c.coef.data();
@@ -90,22 +83,22 @@ static std::vector<float> run(const Case& c, uint64_t seed) {
 
   if (c.iterations > 0)
     launch(seed, blocks(p.segments + 1, kPprThreads), kPprThreads, 0,
-           [&] { ppr_plan_kernel(row_ptr, n, nnz, p.segments, seg_row, head_row); });
-  launch(seed, blocks(n, kPprThreads), kPprThreads, 0, [&] { ppr_init_kernel(reset, d, n, y[0]); });
+           [&] { ppr_plan_kernel(row_ptr, n, nnz, p.segments, p.seg_row, p.head_row); });
+  launch(seed, blocks(n, kPprThreads), kPprThreads, 0, [&] { ppr_init_kernel(reset, d, n, p.y[0]); });
   for (int64_t t = 0; t < c.iterations; ++t) {
-    const float* y_in = y[t & 1];
-    float* y_out = y[(t + 1) & 1];
+    const float* y_in = p.y[t & 1];
+    float* y_out = p.y[(t + 1) & 1];
     launch(seed ? seed + 2 * t : 0, blocks(p.segments, kPprStepWarps), kPprStepThreads, kPprStepSmemBytes, [&] {
-      ppr_step_kernel(row_ptr, col, coef, reset, d, y_in, y_out, seg_row, head_row, n, nnz, p.segments, head_val, carry);
+      ppr_step_kernel(row_ptr, col, coef, reset, d, y_in, y_out, p.seg_row, p.head_row, n, nnz, p.segments, p.head_val, p.carry);
     });
     launch(seed ? seed + 2 * t + 1 : 0, blocks(p.segments, kPprThreads), kPprThreads, 0,
-           [&] { ppr_fixup_kernel(row_ptr, reset, d, head_row, head_val, carry, p.segments, y_out); });
+           [&] { ppr_fixup_kernel(row_ptr, reset, d, p.head_row, p.head_val, p.carry, p.segments, y_out); });
   }
-  const float* y_T = y[c.iterations & 1];
-  launch(seed, unsigned(p.sum_blocks), kPprThreads, kPprSumSmemBytes, [&] { ppr_sum_kernel(y_T, n, partials); });
+  const float* y_T = p.y[c.iterations & 1];
+  launch(seed, unsigned(p.sum_blocks), kPprThreads, kPprSumSmemBytes, [&] { ppr_sum_kernel(y_T, n, p.partials); });
   if (n_out > 0)
     launch(seed, blocks(n_out, kPprThreads), kPprThreads, kPprSumSmemBytes,
-           [&] { ppr_gather_kernel(y_T, partials, p.sum_blocks, out_vertices, n_out, out.data()); });
+           [&] { ppr_gather_kernel(y_T, p.partials, p.sum_blocks, out_vertices, n_out, out.data()); });
   return out;
 }
 

@@ -18,6 +18,7 @@
 
 #include <algorithm>
 #include <functional>
+#include <memory>
 #include <vector>
 
 namespace warp_emu {
@@ -369,6 +370,18 @@ inline void launch_concurrent(unsigned grid, int block, const std::function<void
 }
 
 // kernel<<<grid, block>>>: blocks run one after the other
+// A host stand-in for a device workspace: `bytes` bytes from an `align` boundary, every byte `poison` (0xFF bytes
+// are NaN), so a kernel that reads what it did not write sees garbage.
+struct Workspace {
+  std::vector<uint8_t> mem;
+  uint8_t* base;
+  Workspace(size_t bytes, size_t align, uint8_t poison) : mem(bytes + align, poison) {
+    void* p = mem.data();
+    size_t space = mem.size();
+    base = static_cast<uint8_t*>(std::align(align, bytes, p, space));
+  }
+};
+
 inline void launch(unsigned grid, int block, const std::function<void()>& kernel_call, size_t dynamic_smem_bytes = 0) {
   for (unsigned bidx = 0; bidx < grid; ++bidx) run_block(block, bidx, grid, kernel_call, dynamic_smem_bytes);
 }
