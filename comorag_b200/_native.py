@@ -73,6 +73,9 @@ SIGNATURES = {
     "crag_knn_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
     "crag_knn_topk": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_int,
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "crag_knn_threshold": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_float, C.c_int,
+                                     C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_size_t, C.c_void_p]),
     "crag_ppr_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
     "crag_ppr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_float, C.c_int,
                            C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -12,6 +12,10 @@ Each function keeps the reference method's name, signature, return type and side
 `retrieve_knn` (utils/embed_utils.py:8-97, called at ComoRAG.py:678) is a module-level name and is rebound by
 install() like the other imported names (comorag_b200.retrieval.retrieve_knn).
 
+KNN_METHODS, rebound by install(knn=True) (the default), move the synonymy-edge walk onto the device:
+
+    add_synonymy_edges(self)                        ComoRAG.py:670-712
+
 GRAPH_METHODS, rebound only by install(graph=True), move the graph branch of tri_retrieve onto the device:
 
     graph_search_with_fact_entities(self, query, link_top_k, ...)    ComoRAG.py:992-1055 (+ get_top_k_weights, :972-990)
@@ -20,6 +24,7 @@ GRAPH_METHODS, rebound only by install(graph=True), move the graph branch of tri
 from __future__ import annotations
 
 import logging
+import re
 from typing import Dict, List, Tuple
 
 import numpy as np
@@ -304,6 +309,44 @@ METHODS = {
     "get_query_embeddings": get_query_embeddings,
     "get_fact_scores": get_fact_scores,
     "dense_passage_retrieval": dense_passage_retrieval,
+}
+
+
+# ------------------------------------------------------------------------------------------------ synonymy edges
+# The reference walk accepts while `num_nns > 100` is false (ComoRAG.py:699): at most 101 edges per entity.
+SYNONYMY_CAP = 101
+
+
+def add_synonymy_edges(self) -> None:
+    """ComoRAG.py:670-712 with the k = synonymy_edge_topk kNN lists and their walk replaced by one threshold join
+    (retrieval.synonymy_edges -> crag_knn_threshold): per entity only the edges the walk keeps leave the device.
+    Step for step as the reference: self.entity_id_to_row is set, keys are taken in store order with embeddings from
+    get_embeddings, only entities whose content keeps more than 2 alphanumerics are queries, the entity with content
+    '' is never an edge target, and for each query in key order and each kept edge in rank order
+    `self.node_to_node_stats[(key, nn)] = score` -- so new dict keys land, and existing ones are overwritten, in the
+    reference's order.  The edges are identical to the reference walk over retrieval.retrieve_knn's lists."""
+    logger.info("Expanding graph with synonymy edges")
+    self.entity_id_to_row = self.entity_embedding_store.get_text_for_all_rows()
+    entity_node_keys = list(self.entity_id_to_row.keys())
+    logger.info(f"Performing KNN retrieval for each phrase nodes ({len(entity_node_keys)}).")
+    contents = [self.entity_id_to_row[key]["content"] for key in entity_node_keys]
+    queries = [r for r, text in enumerate(contents) if len(re.sub('[^A-Za-z0-9]', '', text)) > 2]
+    if not queries:
+        return
+    entity_embs = self.entity_embedding_store.get_embeddings(entity_node_keys)
+    empty = [r for r, text in enumerate(contents) if text == '']
+    cfg = self.global_config
+    counts, ids, scores = retrieval.synonymy_edges(entity_embs, queries, cfg.synonymy_edge_sim_threshold, SYNONYMY_CAP,
+                                                   cfg.synonymy_edge_topk, exclude_rows=empty)
+    stats = self.node_to_node_stats
+    for i, r in enumerate(queries):
+        node_key = entity_node_keys[r]
+        for nn, score in zip(ids[i, :counts[i]].tolist(), scores[i, :counts[i]].tolist()):
+            stats[(node_key, entity_node_keys[nn])] = score
+
+
+KNN_METHODS = {
+    "add_synonymy_edges": add_synonymy_edges,
 }
 
 

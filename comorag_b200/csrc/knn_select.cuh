@@ -50,6 +50,30 @@ __device__ __forceinline__ int knn_block_exclusive_scan(int v, int* s_warp, int*
   return before + x - v;
 }
 
+// ---- 3. bitonic sort (descending) of s_keys[0, count), zero-padded to a power of two; ends with the block synced
+__device__ __forceinline__ void knn_bitonic_sort(uint64_t* s_keys, int count, int tid) {
+  int n2 = 1;
+  while (n2 < count) n2 <<= 1;
+  __syncthreads();
+  for (int i = count + tid; i < n2; i += kKnnThreads) s_keys[i] = 0ull;
+  __syncthreads();
+  for (int size = 2; size <= n2; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int p = tid; p < (n2 >> 1); p += kKnnThreads) {
+        const int a = 2 * p - (p & (stride - 1));   // p with a zero bit inserted at `stride`
+        const int b = a + stride;
+        const uint64_t ka = s_keys[a], kb = s_keys[b];
+        const bool desc = (a & size) == 0;
+        if ((ka < kb) == desc) {
+          s_keys[a] = kb;
+          s_keys[b] = ka;
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
+
 // scores: fp32 rows of `ld` floats (ld % 4 == 0, 16-byte aligned), block q reads row q; outputs [gridDim.x, k].
 __global__ void __launch_bounds__(kKnnThreads)
 knn_select_kernel(const float* __restrict__ scores, int64_t ld, int n_rows, int k, int64_t row_offset,
@@ -185,26 +209,7 @@ knn_select_kernel(const float* __restrict__ scores, int64_t ld, int n_rows, int 
   }
 
   // ---- 3. bitonic sort (descending) of the kept keys, zero-padded to a power of two
-  int n2 = 1;
-  while (n2 < count) n2 <<= 1;
-  __syncthreads();
-  for (int i = count + tid; i < n2; i += kKnnThreads) s_keys[i] = 0ull;
-  __syncthreads();
-  for (int size = 2; size <= n2; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int p = tid; p < (n2 >> 1); p += kKnnThreads) {
-        const int a = 2 * p - (p & (stride - 1));   // p with a zero bit inserted at `stride`
-        const int b = a + stride;
-        const uint64_t ka = s_keys[a], kb = s_keys[b];
-        const bool desc = (a & size) == 0;
-        if ((ka < kb) == desc) {
-          s_keys[a] = kb;
-          s_keys[b] = ka;
-        }
-      }
-      __syncthreads();
-    }
-  }
+  knn_bitonic_sort(s_keys, count, tid);
   int64_t* oi = out_ids + int64_t(q) * k;
   float* os = out_scores + int64_t(q) * k;
   for (int j = tid; j < k; j += kKnnThreads) {

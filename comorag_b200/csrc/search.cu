@@ -31,7 +31,8 @@
 // finalize + NVLink exchange + global merge of the row-sharded index
 // (finalize_exchange_kernel), the C-ABI entry points, and crag_knn_topk -- exact
 // top-k up to k = 2048 for large query batches as a score-block GEMM (gemm.cu)
-// plus a per-query radix select (knn_select.cuh).
+// plus a per-query radix select (knn_select.cuh), and crag_knn_threshold -- the same score block, then a per-query
+// threshold join (knn_threshold.cuh).
 #include <type_traits>
 
 #include "common.cuh"
@@ -44,6 +45,7 @@
 #include "select_warps.cuh"
 #include "gemm.cuh"
 #include "knn_select.cuh"
+#include "knn_threshold.cuh"
 #include "workspace.cuh"
 
 namespace crag {
@@ -714,6 +716,43 @@ extern "C" int crag_knn_topk(const void* corpus, int64_t n_rows, int dim, int64_
     knn_select_kernel<<<nqc, kKnnThreads, 0, stream>>>(block, ld, int(n_rows), k, row_offset, out_ids + size_t(q0) * k,
                                                        out_scores + size_t(q0) * k,
                                                        out_minmax ? out_minmax + size_t(q0) * 2 : nullptr);
+    CRAG_CUDA_OK(cudaGetLastError());
+  }
+  return CRAG_OK;
+}
+
+// Threshold join: per chunk of queries the same score block as crag_knn_topk, then knn_threshold_kernel
+// (knn_threshold.cuh) keeps each query's rows scoring >= threshold among its first `limit`, skipping self_rows[q] and
+// exclude_rows, at most `cap` of them.
+extern "C" int crag_knn_threshold(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,
+                                  const void* queries, int nq, float threshold, int limit, int cap,
+                                  const int64_t* self_rows, const int64_t* exclude_rows, int n_exclude,
+                                  int* out_counts, int64_t* out_ids, float* out_scores, void* workspace,
+                                  size_t workspace_bytes, crag_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const Operand c{corpus, n_rows, dim, corpus_row_stride, kBf16, "corpus"}, q{queries, nq, dim, dim, kBf16, "queries"};
+  int rc = check_scan_args("knn_threshold", nq, limit, 0x7FFFFFFF, c, q, workspace, workspace_bytes, 0);
+  if (rc != CRAG_OK) return rc;
+  if (!isfinite(threshold)) return fail(CRAG_ERR_INVALID, "knn_threshold: threshold must be finite");
+  if (cap < 1 || n_exclude < 0 || n_exclude > kKnnMaxExclude || cap + n_exclude + 1 > kKnnMaxK)
+    return fail(CRAG_ERR_INVALID, "knn_threshold: need cap >= 1, 0 <= n_exclude <= %d and cap + n_exclude + 1 <= %d (cap=%d n_exclude=%d)",
+                kKnnMaxExclude, kKnnMaxK, cap, n_exclude);
+  if (!out_counts || !out_ids || !out_scores || (n_exclude > 0 && !exclude_rows)) return fail(CRAG_ERR_INVALID, "knn_threshold: null pointer");
+  const int64_t ld = knn_ld(n_rows);
+  const size_t per_query = size_t(ld) * 4;
+  const size_t fit = workspace_bytes / per_query;
+  if (fit < 1) return fail(CRAG_ERR_WORKSPACE, "knn_threshold: workspace %zu < %zu bytes (one query's score row)", workspace_bytes, per_query);
+  const int q_chunk = fit < size_t(nq) ? int(fit) : nq;
+  float* block = knn_workspace(n_rows, q_chunk, workspace).block;
+  for (int q0 = 0; q0 < nq; q0 += q_chunk) {
+    const int nqc = (nq - q0) < q_chunk ? (nq - q0) : q_chunk;
+    rc = gemm_scores_f32(static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, dim, corpus, corpus_row_stride,
+                         block, ld, nqc, int(n_rows), dim, stream);
+    if (rc != CRAG_OK) return rc;
+    knn_threshold_kernel<<<nqc, kKnnThreads, 0, stream>>>(block, ld, int(n_rows), threshold, limit, cap,
+                                                          self_rows ? self_rows + q0 : nullptr, exclude_rows, n_exclude,
+                                                          out_counts + q0, out_ids + size_t(q0) * cap,
+                                                          out_scores + size_t(q0) * cap);
     CRAG_CUDA_OK(cudaGetLastError());
   }
   return CRAG_OK;

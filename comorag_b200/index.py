@@ -48,6 +48,16 @@ def knn_chunk(nq: int, n_rows: int, budget: int = KNN_WORKSPACE_BYTES) -> int:
     return c
 
 
+def fp32_threshold(t: float) -> float:
+    """The smallest fp32 value >= the double t.  A score s (fp32) passes `s >= t` compared as doubles exactly when it
+    passes `s >= fp32_threshold(t)` compared as fp32 -- the form crag_knn_threshold takes its threshold in.  At 0.8
+    this is float32(0.8), which rounds up; at 0.7 float32(0.7) rounds down and the next fp32 above it is returned."""
+    f = np.float32(t)
+    if float(f) < float(t):
+        f = np.nextafter(f, np.float32(np.inf))
+    return float(f)
+
+
 def use_knn(nq: int, n_rows: int, k: int) -> bool:
     """Route a search to crag_knn_topk (True) or to the shard scan (False): for k <= 2048, the GEMM path for large
     query batches whose chunks stay large, or for k >= KNN_MIN_K_FEW; the scan otherwise and always beyond k = 2048."""
@@ -323,6 +333,46 @@ class DenseIndex:
                     minmax.data_ptr(), ws.data_ptr(), ws_bytes, st.cuda_stream)
                 _native.check(rc, "crag_knn_topk")
         return ids, scores, minmax
+
+    def search_threshold_device(self, queries: torch.Tensor, threshold: float, cap: int, limit: int,
+                                self_rows: Optional[torch.Tensor] = None, exclude_rows=None,
+                                stream: Optional[torch.cuda.Stream] = None
+                                ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Threshold join (crag_knn_threshold) of a device bf16 [nq, dim_pad] query block: for each query, walk the
+        first `limit` rows of its crag_knn_topk list, stop at the first scoring below `threshold` (an fp32 value: see
+        fp32_threshold), skip self_rows[q] (int64 [nq] local rows, -1 for none) and `exclude_rows` (at most 64 local
+        rows), and keep the others, at most `cap`.  Returns (counts int32 [nq], ids int64 [nq, cap] local rows,
+        scores fp32 [nq, cap]) on the device, -1 / -inf past each count.  Single shard; chunks queries as
+        _search_device_knn does."""
+        if queries.dtype != torch.bfloat16 or queries.dim() != 2 or queries.shape[1] != self.dim_pad:
+            raise ValueError(f"queries must be bf16 [nq, {self.dim_pad}]")
+        queries = queries.contiguous()
+        nq = queries.shape[0]
+        lib = _native.load()
+        dev = self.device
+        buf, n_rows = self._snapshot()
+        with torch.cuda.device(dev):
+            st = stream if stream is not None else torch.cuda.current_stream(dev)
+            with torch.cuda.stream(st):
+                excl = torch.as_tensor(list(exclude_rows) if exclude_rows is not None else [], dtype=torch.int64)
+                excl = excl.to(dev, non_blocking=True)
+                selfr = None
+                if self_rows is not None:
+                    selfr = torch.as_tensor(self_rows, dtype=torch.int64).to(dev, non_blocking=True).contiguous()
+                    if selfr.shape != (nq,):
+                        raise ValueError(f"self_rows must hold one row per query ({nq})")
+                counts = torch.empty((nq,), dtype=torch.int32, device=dev)
+                ids = torch.empty((nq, cap), dtype=torch.int64, device=dev)
+                scores = torch.empty((nq, cap), dtype=torch.float32, device=dev)
+                ws_bytes = lib.crag_knn_workspace_bytes(n_rows, knn_chunk(max(nq, 1), n_rows))
+                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+                rc = lib.crag_knn_threshold(
+                    buf.data_ptr() if n_rows else 0, n_rows, self.dim_pad,
+                    buf.stride(0) if buf.shape[0] else self.dim_pad, queries.data_ptr(), nq, float(threshold),
+                    int(limit), int(cap), _native.ptr(selfr), excl.data_ptr() if excl.numel() else 0, excl.numel(),
+                    counts.data_ptr(), ids.data_ptr(), scores.data_ptr(), ws.data_ptr(), ws_bytes, st.cuda_stream)
+                _native.check(rc, "crag_knn_threshold")
+        return counts, ids, scores
 
     def _search_device_paged(self, queries: torch.Tensor, k: int, stream: Optional[torch.cuda.Stream]):
         """k > 128 where crag_knn_topk does not pay off (few queries, or k > 2048): ceil(k/128) passes chained with

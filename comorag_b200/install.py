@@ -24,7 +24,10 @@ def install(package: str = "src.comorag", rerank: bool = False, summaries: bool 
             umap: bool = False) -> Dict[str, int]:
     """Returns {name: number of module attributes (or class methods) rebound}.  `rerank=True` also swaps the LLM
     filter for the dense reranker (new arithmetic, off by default so answers stay reference-identical); `search`
-    rebinds the four ComoRAG retrieval methods, `knn` the synonymy-edge retrieve_knn; `encoder=False` keeps the
+    rebinds the four ComoRAG retrieval methods; `knn` puts the synonymy-edge kNN on the device: it rebinds
+    retrieve_knn (crag_knn_topk, for any caller) and ComoRAG.add_synonymy_edges (comorag_methods.KNN_METHODS: one
+    threshold join, crag_knn_threshold, returns only the edges the reference walk keeps, identical to that walk over
+    retrieve_knn's k = synonymy_edge_topk lists); `encoder=False` keeps the
     reference's own embedding model class (HF, fp32) and swaps only the store / search half -- the parity tests use
     that to compare rankings without the bf16 encoder's error in the way.  `graph=True` also rebinds
     graph_search_with_fact_entities and run_ppr (comorag_methods.GRAPH_METHODS: PPR on the device, crag_ppr); it
@@ -61,11 +64,12 @@ def install(package: str = "src.comorag", rerank: bool = False, summaries: bool 
             if getattr(mod, attr, None) is old:
                 setattr(mod, attr, new)
                 counts[attr] += 1
-    if search or graph:
+    if search or graph or knn:
         from . import comorag_methods as cm
         main = sys.modules.get(package + ".ComoRAG") or importlib.import_module(package + ".ComoRAG")
         cls = main.ComoRAG
-        methods = {**(cm.METHODS if search else {}), **(cm.GRAPH_METHODS if graph else {})}
+        methods = {**(cm.METHODS if search else {}), **(cm.GRAPH_METHODS if graph else {}),
+                   **(cm.KNN_METHODS if knn else {})}
         originals = cls.__dict__.get("_comorag_b200_originals")
         if originals is None:
             originals = {}

@@ -11,7 +11,7 @@ from typing import List, Optional, Tuple
 
 import numpy as np
 
-from .index import DenseIndex, MAX_K
+from .index import DenseIndex, MAX_K, fp32_threshold
 
 
 def min_max_normalize(x: np.ndarray) -> np.ndarray:
@@ -106,6 +106,37 @@ def get_similar_summaries(query: str, level_store, embedding_model, top_k: int =
     return [level_store.texts[i] for i in ids[0] if i >= 0], [float(s) for s, i in zip(norm, ids[0]) if i >= 0]
 
 
+def knn_key_index(key_vecs, device=None) -> DenseIndex:
+    """The key shard of retrieve_knn: rows L2-normalised in fp32 (embed_utils.py:8-97 normalises both sides), then
+    stored as bf16 by DenseIndex.add.  synonymy_edges builds its shard here too, so both see the same words."""
+    import torch
+    kv = torch.nn.functional.normalize(torch.as_tensor(np.asarray(key_vecs), dtype=torch.float32), dim=1)
+    index = DenseIndex(kv.shape[1], device=device, capacity=kv.shape[0])
+    index.add(kv)
+    return index
+
+
+def synonymy_edges(key_vecs, query_rows, threshold: float, cap: int, limit: int, exclude_rows=(), device=None,
+                   stream=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """The self-join of add_synonymy_edges as a threshold join: the keys go to a shard (knn_key_index), the queries are
+    the stored rows `query_rows` of that shard (the same bf16 words retrieve_knn would send), and crag_knn_threshold
+    returns, per query, the keys walk ComoRAG.py:698-710 keeps from retrieve_knn(k=limit)'s list: scores >= the
+    double `threshold` in rank order, the query's own row and `exclude_rows` skipped, at most `cap`.  Returns host
+    (counts int32 [nq], ids int64 [nq, w] key rows, scores fp32 [nq, w]), w = the largest count; only those columns
+    leave the device."""
+    import torch
+    index = knn_key_index(key_vecs, device)
+    rows = torch.as_tensor(np.asarray(query_rows, dtype=np.int64))
+    with torch.cuda.device(index.device):
+        rows_d = rows.to(index.device)
+        q = index._buf[: index.n_rows].index_select(0, rows_d)
+        counts, ids, scores = index.search_threshold_device(q, fp32_threshold(threshold), cap, limit, self_rows=rows_d,
+                                                            exclude_rows=exclude_rows, stream=stream)
+        counts_h = counts.cpu().numpy()
+        w = int(counts_h.max()) if counts_h.size else 0
+        return counts_h, ids[:, :w].cpu().numpy(), scores[:, :w].cpu().numpy()
+
+
 def retrieve_knn(query_ids: List[str], key_ids: List[str], query_vecs, key_vecs, k: int = 2047,
                  query_batch_size: int = 1000, key_batch_size: int = 10000, device=None):
     """embed_utils.py:8-97: top-k most similar keys (cosine) for every query -> {query_id: (key ids, scores)}.
@@ -122,10 +153,8 @@ def retrieve_knn(query_ids: List[str], key_ids: List[str], query_vecs, key_vecs,
     if len(key_vecs) == 0:
         return {}
     q = torch.nn.functional.normalize(torch.as_tensor(np.asarray(query_vecs), dtype=torch.float32), dim=1)
-    kv = torch.nn.functional.normalize(torch.as_tensor(np.asarray(key_vecs), dtype=torch.float32), dim=1)
-    index = DenseIndex(kv.shape[1], device=device, capacity=kv.shape[0])
-    index.add(kv)
-    kk = min(int(k), kv.shape[0])
+    index = knn_key_index(key_vecs, device)
+    kk = min(int(k), index.n_rows)
     results = {}
     step = 1024  # queries per launch group (32 per corpus pass inside the library)
     for s0 in range(0, q.shape[0], step):

@@ -155,6 +155,20 @@ CRAG_API int crag_knn_topk(const void* corpus, int64_t n_rows, int dim, int64_t 
                            const void* queries, int nq, int k, int64_t* out_ids, float* out_scores, float* out_minmax,
                            void* workspace, size_t workspace_bytes, crag_stream_t stream);
 
+/* Threshold join on crag_knn_topk's score block (same workspace, sized by crag_knn_workspace_bytes): for query q, walk
+ * the first min(limit, n_rows) rows in crag_knn_topk's order, stop at the first with !(score >= threshold), skip
+ * self_rows[q] (a local row or -1; self_rows may be null) and every row of exclude_rows, and keep the others until
+ * `cap` are kept -- the synonymy-edge loop of the reference's add_synonymy_edges (ComoRAG.py:689-712) without the
+ * k = 2047 lists.  Outputs: out_counts int32 [nq] in [0, cap], out_ids int64 (local rows) / out_scores fp32 [nq, cap]
+ * in rank order, -1 / -inf past the count.  Argument rules of crag_knn_topk for the operands and the workspace, any
+ * limit >= 1, and CRAG_ERR_INVALID for a non-finite threshold, cap < 1, n_exclude outside [0, 64] or
+ * cap + n_exclude + 1 > 2048.  A caller holding a double threshold t passes the smallest fp32 >= t. */
+CRAG_API int crag_knn_threshold(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,
+                                const void* queries, int nq, float threshold, int limit, int cap,
+                                const int64_t* self_rows, const int64_t* exclude_rows, int n_exclude,
+                                int* out_counts, int64_t* out_ids, float* out_scores, void* workspace,
+                                size_t workspace_bytes, crag_stream_t stream);
+
 /* The two halves of crag_search_topk for ONE pass (nq <= 32), exported so a caller can time or overlap them:
  * crag_search_scan streams the shard once and leaves per-CTA partial lists in the workspace;
  * crag_search_finalize merges them into (ids, scores, minmax).  Same argument rules as crag_search_topk. */
