@@ -97,6 +97,13 @@ SIGNATURES = {
                                      C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "crag_ivf_pq_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int, C.c_int]),
+    "crag_ivf_search_pq": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
+                                     C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,
+                                     C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "crag_pq_encode": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
+                                 C.c_void_p]),
     "crag_gmm_sweep_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
     "crag_gmm_sweep": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -32,7 +32,9 @@
 // (finalize_exchange_kernel), the C-ABI entry points, and crag_knn_topk -- exact
 // top-k up to k = 2048 for large query batches as a score-block GEMM (gemm.cu)
 // plus a per-query radix select (knn_select.cuh), and crag_knn_threshold -- the same score block, then a per-query
-// threshold join (knn_threshold.cuh).
+// threshold join (knn_threshold.cuh).  crag_ivf_search_pq runs the IVF plan, then the PQ table and scan kernels
+// (pq_kernels.cuh), then the same merge, rescore and id map as crag_ivf_search_i8.
+#include <algorithm>
 #include <type_traits>
 
 #include "common.cuh"
@@ -46,6 +48,7 @@
 #include "gemm.cuh"
 #include "knn_select.cuh"
 #include "knn_threshold.cuh"
+#include "pq_kernels.cuh"
 #include "workspace.cuh"
 
 namespace crag {
@@ -609,6 +612,155 @@ extern "C" int crag_ivf_search_i8(const void* residuals_i8, const float* row_sca
   rescore.cand_scores = plan.cand_scores;
   return ivf_passes(res, q, I8IvfArgs{{}, {row_scales, query_scales}}, lists, n_cand, k, &rescore, out_ids, out_scores, out_minmax, plan.ivf,
                     static_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------ IVF over product-quantized residuals (pq_kernels.cuh)
+namespace crag {
+namespace {
+
+// PQ IVF workspace = the int8 IVF workspace for n_cand candidates, then the tables of one pass's queries
+struct IvfPqPlan {
+  IvfI8Plan cand;
+  float* lut;   // [kNQ][m][256]
+  size_t total;
+};
+IvfPqPlan plan_ivf_pq(int nlist, int64_t total_tiles, int n_cand, int m, const void* ws = nullptr) {
+  IvfPqPlan p;
+  p.cand = plan_ivf_i8(nlist, total_tiles, n_cand, ws);
+  WsCursor c(ws, p.cand.total);
+  p.lut = c.take<float>(size_t(kNQ) * m * kPqCodewords);
+  p.total = c.bytes;
+  return p;
+}
+
+int check_pq_shape(const char* who, int dim, int m) {
+  if (dim < 64 || dim > 1024 || dim % 64 != 0) return fail(CRAG_ERR_INVALID, "%s: dim must be a multiple of 64 in [64, 1024] (dim=%d)", who, dim);
+  if (m < 1 || m > kPqMaxM || dim % m != 0 || dim / m > kPqMaxDsub) return fail(CRAG_ERR_INVALID, "%s: m must divide dim with 1 <= m <= %d and dim / m <= %d (dim=%d m=%d)", who, kPqMaxM, kPqMaxDsub, dim, m);
+  return CRAG_OK;
+}
+
+// The dynamic shared-memory limit of a kernel is raised once per device, to what its largest shape needs.
+template <class Kernel>
+int allow_smem(Kernel kern, size_t bytes, bool (&done)[64]) {
+  int dev = 0;
+  CRAG_CUDA_OK(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64 || !done[dev]) {
+    CRAG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes)));
+    if (dev >= 0 && dev < 64) done[dev] = true;
+  }
+  return CRAG_OK;
+}
+
+// Every 32-query pass of a PQ IVF search: the plan, the queries' tables, the PQ scan for n_cand candidates, the merge
+// of its partials, the exact rescore of the candidates and the map of stored positions to original ids.
+int ivf_pq_passes(const uint8_t* codes, int64_t code_stride, int m, const float* codebooks, const IvfLists& l,
+                  int n_cand, int k, const IvfRescore& rescore, int64_t* out_ids, float* out_scores, float* out_minmax,
+                  const IvfPqPlan& pp, cudaStream_t stream) {
+  const IvfPlan& ip = pp.cand.ivf;
+  const SearchPlan& sp = ip.scan;
+  const IvfArgs args{ip.work, ip.n_work, ip.list_mask, ip.coarse};
+  const int nq = int(rescore.queries.rows), dim = rescore.queries.width;
+  for (int q0 = 0; q0 < nq; q0 += kNQ) {
+    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
+    ivf_plan_kernel<<<1, 1024, 0, stream>>>(l.probed_ids + size_t(q0) * l.nprobe, l.probed_scores + size_t(q0) * l.nprobe, nqc,
+                                            l.nprobe, l.nlist, l.tile_start, l.rows, ip.list_mask, ip.coarse, ip.work,
+                                            ip.n_work);
+    CRAG_CUDA_OK(cudaGetLastError());
+    const void* qp = rescore.queries.rows_from(q0, nqc).ptr;
+    pq_table_kernel<<<unsigned(nqc * m), kPqTableThreads, 0, stream>>>(static_cast<const uint16_t*>(qp), dim, codebooks, m, pp.lut);
+    CRAG_CUDA_OK(cudaGetLastError());
+    // about two CTAs per SM in all; every (slice, query) CTA writes its part, so the merge reads `slices` parts
+    const int slices = std::min(sp.grid, std::max(1, (2 * sp.grid + nqc - 1) / nqc));
+    int rc = CRAG_OK;
+    with_merge_tier(n_cand, [&](auto tier) {
+      constexpr int T = decltype(tier)::value;
+      static bool attr_set[64] = {};
+      rc = allow_smem(pq_scan_kernel<T>, PqScanSmem<T>::bytes(kPqMaxM), attr_set);
+      if (rc != CRAG_OK) return;
+      pq_scan_kernel<T><<<unsigned(nqc * slices), kPqThreads, PqScanSmem<T>::bytes(m), stream>>>(
+          codes, code_stride, m, pp.lut, slices, n_cand, args, sp.part_keys, sp.part_minmax);
+    });
+    if (rc != CRAG_OK) return rc;
+    CRAG_CUDA_OK(cudaGetLastError());
+    float* minmax = out_minmax ? out_minmax + size_t(q0) * 2 : nullptr;
+    int64_t* ids = out_ids + size_t(q0) * k;
+    rc = finalize_parts(slices, nqc, n_cand, 0, pp.cand.cand_ids, pp.cand.cand_scores, minmax, nullptr, sp, stream);
+    if (rc == CRAG_OK)
+      rc = launch_ivf_rescore(rescore.rows.ptr, rescore.rows.rows, rescore.rows.width, rescore.rows.stride, qp, nqc,
+                              pp.cand.cand_ids, n_cand, k, l.tile_start, l.nlist, ip.coarse, ids,
+                              out_scores + size_t(q0) * k, stream);
+    if (rc != CRAG_OK) return rc;
+    ivf_map_ids_kernel<<<(nqc * k + 255) / 256, 256, 0, stream>>>(ids, nqc * k, l.row_ids);
+    CRAG_CUDA_OK(cudaGetLastError());
+  }
+  return CRAG_OK;
+}
+
+}  // namespace
+}  // namespace crag
+
+extern "C" size_t crag_ivf_pq_workspace_bytes(int nlist, int64_t total_tiles, int n_cand, int m) {
+  if (nlist < 1 || total_tiles < 0 || n_cand < 1 || n_cand > 128 || m < 1 || m > kPqMaxM) return 0;
+  return plan_ivf_pq(nlist, total_tiles, n_cand, m).total;
+}
+
+extern "C" int crag_ivf_search_pq(const void* codes, int m, int64_t code_stride, const float* codebooks,
+                                  const void* residuals_bf16, int dim, int64_t row_stride, int64_t n_rows_padded,
+                                  const int32_t* list_tile_start, const int32_t* list_rows, int nlist,
+                                  int64_t total_tiles, const int64_t* row_ids, const void* queries_bf16, int nq,
+                                  const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand, int k,
+                                  int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                                  size_t workspace_bytes, crag_stream_t stream) {
+  IvfRescore rescore{{residuals_bf16, n_rows_padded, dim, row_stride, kBf16, "residuals_bf16"},
+                     {queries_bf16, nq, dim, dim, kBf16, "queries_bf16"}, nullptr, nullptr};
+  const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
+  int rc = check_ivf_args("ivf_pq", lists, n_rows_padded, out_ids, out_scores);
+  if (rc != CRAG_OK) return rc;
+  if (nq < 1 || k < 1 || n_cand < k || n_cand > 128) return fail(CRAG_ERR_INVALID, "ivf_pq: need nq >= 1 and 1 <= k <= n_cand <= 128 (nq=%d k=%d n_cand=%d)", nq, k, n_cand);
+  rc = check_pq_shape("ivf_pq", dim, m);
+  if (rc != CRAG_OK) return rc;
+  if (code_stride < pq_code_stride(m) || code_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "ivf_pq: code_stride must be a multiple of 16 and >= %d (code_stride=%lld)", pq_code_stride(m), (long long)code_stride);
+  if (!codes || !codebooks) return fail(CRAG_ERR_INVALID, "ivf_pq: null codes or codebooks pointer");
+  if ((reinterpret_cast<uintptr_t>(codes) | reinterpret_cast<uintptr_t>(codebooks)) & 15) return fail(CRAG_ERR_INVALID, "ivf_pq: codes and codebooks must be 16-byte aligned");
+  rc = check_operand("ivf_pq", rescore.rows);
+  if (rc == CRAG_OK) rc = check_operand("ivf_pq", rescore.queries);
+  const IvfPqPlan plan = plan_ivf_pq(nlist, total_tiles, n_cand, m, workspace);
+  if (rc == CRAG_OK) rc = check_workspace("ivf_pq", workspace, workspace_bytes, plan.total);
+  if (rc != CRAG_OK) return rc;
+  // the bf16 residuals may be page-locked host memory: refused before any launch if pageable
+  rc = device_readable(residuals_bf16, &rescore.rows.ptr, "ivf_pq");
+  if (rc != CRAG_OK) return rc;
+  return ivf_pq_passes(static_cast<const uint8_t*>(codes), code_stride, m, codebooks, lists, n_cand, k, rescore, out_ids,
+                       out_scores, out_minmax, plan, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int crag_pq_encode(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, const float* codebooks,
+                              int m, void* codes, int64_t code_stride, crag_stream_t stream) {
+  int rc = check_pq_shape("pq_encode", dim, m);
+  if (rc != CRAG_OK) return rc;
+  if (n_rows < 0 || n_rows >= (int64_t(1) << 31)) return fail(CRAG_ERR_INVALID, "pq_encode: n_rows out of range (%lld)", (long long)n_rows);
+  if (row_stride < dim) return fail(CRAG_ERR_INVALID, "pq_encode: row_stride must be >= dim (row_stride=%lld dim=%d)", (long long)row_stride, dim);
+  if (code_stride < m) return fail(CRAG_ERR_INVALID, "pq_encode: code_stride must be >= m (code_stride=%lld m=%d)", (long long)code_stride, m);
+  if (n_rows == 0) return CRAG_OK;
+  if (!rows_bf16 || !codebooks || !codes) return fail(CRAG_ERR_INVALID, "pq_encode: null rows, codebooks or codes pointer");
+  if ((reinterpret_cast<uintptr_t>(rows_bf16) & 1) || (reinterpret_cast<uintptr_t>(codebooks) & 3)) return fail(CRAG_ERR_INVALID, "pq_encode: rows must be 2-byte and codebooks 4-byte aligned");
+  const void* rows = rows_bf16;
+  rc = device_readable(rows_bf16, &rows, "pq_encode");
+  if (rc != CRAG_OK) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  static bool attr_set[64] = {};
+  rc = allow_smem(pq_encode_kernel, pq_encode_smem_bytes(kPqMaxDsub), attr_set);
+  if (rc != CRAG_OK) return rc;
+  constexpr int64_t kChunk = int64_t(1) << 22;   // rows per launch: (chunk / 128) * m blocks stay far below 2^31
+  for (int64_t r0 = 0; r0 < n_rows; r0 += kChunk) {
+    const int64_t n = std::min(kChunk, n_rows - r0);
+    const unsigned grid = unsigned((n + kPqThreads - 1) / kPqThreads) * unsigned(m);
+    pq_encode_kernel<<<grid, kPqThreads, pq_encode_smem_bytes(dim / m), st>>>(
+        static_cast<const uint16_t*>(rows) + r0 * row_stride, n, dim, row_stride, codebooks, m,
+        static_cast<uint8_t*>(codes) + r0 * code_stride, code_stride);
+    CRAG_CUDA_OK(cudaGetLastError());
+  }
+  return CRAG_OK;
 }
 
 extern "C" int crag_search_scan(const void* corpus, int64_t n_rows, int dim, int64_t corpus_row_stride,

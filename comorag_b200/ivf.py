@@ -304,7 +304,8 @@ class ShardedIVF:
       position is >= that index's: the global top `candidates` by S1 lie inside the union of the ranks'."""
 
     def __init__(self, local, group=None):
-        """`local`: this rank's IVFIndex or QuantizedIVF."""
+        """`local`: this rank's IVFIndex, QuantizedIVF or pq.PQIVF (a PQIVF rescores its own candidates, as a
+        QuantizedIVF does)."""
         import torch.distributed as dist
         self.local, self.group = local, group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1

@@ -348,6 +348,37 @@ CRAG_API int crag_ivf_search_i8(const void* residuals_i8, const float* row_scale
                                 int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
                                 size_t workspace_bytes, crag_stream_t stream);
 
+/* IVF over product-quantized residuals: crag_ivf_search's shard layout with every stored residual row also encoded by
+ * crag_pq_encode as m one-byte codes, one per subspace of dsub = dim / m columns.  Per block of 32 queries, in one call:
+ * the IVF plan; each query's table LUT_q[j][c] = sum_t q_{j,t} C_j[c][t] (fp32, t order, no FMA); a scan of the
+ * probed tiles' codes keeping the top n_cand stored positions by
+ *   S1 = (sum_j LUT_q[j][code_j]) + (q . c_list)        (fp32 adds rounded to nearest, j order, coarse term last)
+ * ties by ascending position; then crag_ivf_search_i8's exact rescore, S2 = dot + (q . c_list), and id map.  -1 / -inf
+ * past the valid candidates; out_minmax (may be NULL) is (min, max) of S1 over the probed rows, (+inf, -inf) when
+ * there are none.  When the int8 and the PQ stage keep the same candidates, the answers are bit-identical.  Semantics
+ * in DESIGN.md section 7.
+ *   codes      device uint8 [n_rows_padded, code_stride], code_stride a multiple of 16 and >= m rounded up to 16
+ *   codebooks  device fp32 [m, 256, dsub] dense, 16-byte aligned; m divides dim, 1 <= m <= 192, dsub <= 128
+ *   residuals_bf16  bf16 [n_rows_padded, row_stride], device or page-locked host memory (pageable: CRAG_ERR_INVALID
+ *              before any launch); dim a multiple of 64 in [64, 1024]; queries_bf16 device bf16 [nq, dim] dense
+ *   list layout, row_ids, probed_ids / probed_scores, nprobe as crag_ivf_search; 1 <= k <= n_cand <= 128.
+ * workspace >= crag_ivf_pq_workspace_bytes(nlist, total_tiles, n_cand, m), 256-byte aligned (0 for bad arguments). */
+CRAG_API size_t crag_ivf_pq_workspace_bytes(int nlist, int64_t total_tiles, int n_cand, int m);
+CRAG_API int crag_ivf_search_pq(const void* codes, int m, int64_t code_stride, const float* codebooks,
+                                const void* residuals_bf16, int dim, int64_t row_stride, int64_t n_rows_padded,
+                                const int32_t* list_tile_start, const int32_t* list_rows, int nlist,
+                                int64_t total_tiles, const int64_t* row_ids, const void* queries_bf16, int nq,
+                                const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand, int k,
+                                int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                                size_t workspace_bytes, crag_stream_t stream);
+/* Product-quantizer encode (also the assignment step of codebook training): for every row r and subspace j,
+ * codes[r * code_stride + j] = argmin_c sum_t (r_{j,t} - C_j[c][t])^2 over the bf16 row read as fp32 (fp32, t order,
+ * no FMA, ties to the smaller c).  rows bf16 [n_rows, row_stride] (device or page-locked host memory); codebooks device
+ * fp32 [m, 256, dsub] dense; codes device uint8 [n_rows, code_stride >= m]; bytes m .. code_stride - 1 are not
+ * written.  dim and m as crag_ivf_search_pq. */
+CRAG_API int crag_pq_encode(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, const float* codebooks,
+                            int m, void* codes, int64_t code_stride, crag_stream_t stream);
+
 /* IVF build, assignment step: best_id[r] = argmax_l bf16(row r) . bf16(centroid l) (fp32 accumulation on the tensor
  * cores, ties to the smaller l), best_score[r] = that inner product.  rows device bf16 [n_rows, dim] (row_stride
  * elements), centroids device bf16 [nlist, dim] contiguous; outputs device fp32 / int32 [n_rows].  nlist / 32 passes of
