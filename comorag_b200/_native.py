@@ -92,6 +92,11 @@ SIGNATURES = {
                                       C.c_size_t, C.c_void_p]),
     "crag_rescore_topk": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_int,
                                     C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crag_binarize_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                     C.c_void_p]),
+    "crag_search_topk_b1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_void_p,
+                                      C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_size_t, C.c_void_p]),
     "crag_ivf_i8_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int]),
     "crag_ivf_search_i8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int64,
                                      C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,

@@ -179,6 +179,18 @@ __device__ __forceinline__ void wgmma_m64n32k32_s8_ss(int32_t (&d)[16], uint64_t
       : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
       : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
+// Register-A form: D[64 x 32] (+)= A[64 x 32] (registers, 4 s8 per register in the m64nNk32 A layout, binary.cuh) .
+// B[32 x 32]^T (smem, K-major, sw128).  The A registers are read asynchronously: they must not be written again until
+// a wgmma_wait has retired this wgmma's group.
+__device__ __forceinline__ void wgmma_m64n32k32_s8_rs(int32_t (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate));
+}
 // wgmma_fence_regs for s32 accumulators
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(int32_t (&d)[R]) {

@@ -1,4 +1,5 @@
-// Int8 corpus shards: C entries of the quantiser and of the exact bf16 rescore (quant_kernels.cuh).  The int8 scan
+// Int8 and one-bit corpus shards: C entries of the quantiser, the binariser and the exact bf16 rescore
+// (quant_kernels.cuh).  The int8 scan
 // between them, crag_search_topk_i8, is the I8 variant of the shard scan in search.cu.  The int8 IVF search
 // (crag_ivf_search_i8, search.cu) launches its rescore through launch_ivf_rescore here, so that the rescore kernels
 // have one translation unit.
@@ -54,6 +55,23 @@ extern "C" int crag_quantize_rows_i8(const void* rows_bf16, int64_t n_rows, int 
   const int64_t grid = (n_rows + kQuantThreads / 32 - 1) / (kQuantThreads / 32);
   quantize_rows_kernel<<<unsigned(grid), kQuantThreads, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint16_t*>(rows_bf16), n_rows, dim, row_stride, dim8, static_cast<int8_t*>(out_i8), out_stride, out_scales);
+  CRAG_CUDA_OK(cudaGetLastError());
+  return CRAG_OK;
+}
+
+extern "C" int crag_binarize_rows(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, void* out_bits,
+                                  int64_t out_stride, float* out_alpha, crag_stream_t stream) {
+  if (dim < 1 || dim > 1024) return fail(CRAG_ERR_INVALID, "binarize: dim must be in [1, 1024] (dim=%d)", dim);
+  const int dim8 = (dim + 127) / 128 * 128;
+  if (n_rows < 0 || n_rows >= (int64_t(1) << 31)) return fail(CRAG_ERR_INVALID, "binarize: n_rows out of range (%lld)", (long long)n_rows);
+  if (row_stride < dim) return fail(CRAG_ERR_INVALID, "binarize: row_stride must be >= dim");
+  if (out_stride < dim8 / 8 || out_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "binarize: out_stride must be >= %d bytes and a multiple of 16", dim8 / 8);
+  if (n_rows == 0) return CRAG_OK;
+  if (!rows_bf16 || !out_bits || !out_alpha) return fail(CRAG_ERR_INVALID, "binarize: null rows, out_bits or out_alpha pointer");
+  if ((reinterpret_cast<uintptr_t>(rows_bf16) & 1) || (reinterpret_cast<uintptr_t>(out_bits) & 15)) return fail(CRAG_ERR_INVALID, "binarize: rows must be 2-byte and out_bits 16-byte aligned");
+  const int64_t grid = (n_rows + kBinarizeThreads / 32 - 1) / (kBinarizeThreads / 32);
+  binarize_rows_kernel<<<unsigned(grid), kBinarizeThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint16_t*>(rows_bf16), n_rows, dim, row_stride, dim8, static_cast<uint8_t*>(out_bits), out_stride, out_alpha);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }

@@ -9,6 +9,10 @@
 //             is added to the lane's partial (rounded) in element order from 0.f; the partials are combined by an
 //             xor-shuffle tree over 16, 8, 4, 2, 1.  The result is the top k of the candidates by (score descending,
 //             row ascending), as make_key orders them.
+//   binarize  (one-bit shards, crag_search_topk_b1, DESIGN.md 3f) a bf16 row x of width dim becomes dim8 / 8 code bytes,
+//             bit j of byte b set iff x_(8 b + j) > 0 (zeros, -0 and the padding columns dim .. dim8 - 1 give 0, read as
+//             -1), and alpha = sum |x_i| / dim (division rounded to nearest), the sum taken in the rescore's order
+//             below; alpha = 0 for a zero row.
 //   IVF       (crag_ivf_search_i8, DESIGN.md 7) the candidates are stored positions p of an IVF shard's padded residual
 //             array; p's list l is the one with list_tile_start[l] <= p / 128 < list_tile_start[l + 1], and its score
 //             is fadd(dot, coarse[l][q]) with the pass's coarse table (ivf_plan_kernel).
@@ -67,6 +71,34 @@ quantize_rows_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim,
     *reinterpret_cast<uint32_t*>(o + c0) = packed;
   }
   if (lane == 0) scales[row] = s;
+}
+
+constexpr int kBinarizeThreads = 256;        // binarize: one warp per row
+
+// rows: bf16 bits [n_rows, row_stride], dim valid columns.  bits: [n_rows, out_stride] bytes, dim8 / 8 written (dim8 a
+// multiple of 128, bits 4-byte aligned, out_stride a multiple of 4); alpha: fp32 [n_rows].
+__global__ void __launch_bounds__(kBinarizeThreads)
+binarize_rows_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride, int dim8,
+                     uint8_t* __restrict__ bits, int64_t out_stride, float* __restrict__ alpha) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = int64_t(blockIdx.x) * (kBinarizeThreads / 32) + (threadIdx.x >> 5);
+  if (row >= n_rows) return;   // warp-uniform
+  const uint16_t* x = rows + row * row_stride;
+  // sum |x_i|: lane l adds the 8-column chunks l, l + 32, ... in element order, then an xor tree over the lanes
+  float abs_sum = 0.f;
+  for (int c0 = lane * 8; c0 < dim; c0 += 32 * 8)
+    for (int c = c0; c < c0 + 8 && c < dim; ++c) abs_sum = __fadd_rn(abs_sum, bf16_bits_to_f32(x[c] & 0x7FFFu));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) abs_sum = __fadd_rn(abs_sum, __shfl_xor_sync(0xffffffffu, abs_sum, o));
+  // code word w: lane j's column 32 w + j in bit j; positive = sign clear and not zero
+  uint32_t* out = reinterpret_cast<uint32_t*>(bits + row * out_stride);
+  for (int w = 0; w < dim8 / 32; ++w) {
+    const int c = 32 * w + lane;
+    const uint32_t v = c < dim ? x[c] : 0u;
+    const uint32_t word = __ballot_sync(0xffffffffu, v != 0u && v < 0x8000u);
+    if (lane == (w & 31)) out[w] = word;
+  }
+  if (lane == 0) alpha[row] = __fdiv_rn(abs_sum, float(dim));
 }
 
 // partial += a_i * b_i over the 8 bf16 of one 16-byte chunk, in element order (the low half of a word comes first)

@@ -26,7 +26,8 @@
 // The shard is read exactly once from HBM: algorithmic bytes = n_rows*dim*2.
 // Variants of the same pipeline, named by the kernel's argument struct: IvfArgs walks a work-list of probed tiles
 // (crag_ivf_search); ScoreArgs stores every score (crag_search_scores) or keeps each row's running argmax over centroid
-// blocks (crag_ivf_assign); I8Args scans int8 rows (crag_search_topk_i8), I8IvfArgs int8 IVF lists (crag_ivf_search_i8).
+// blocks (crag_ivf_assign); I8Args scans int8 rows (crag_search_topk_i8), I8IvfArgs int8 IVF lists (crag_ivf_search_i8),
+// B1Args one-bit rows (crag_search_topk_b1).
 // Around it in this file: the per-shard merge (merge_topk_kernel), the fused
 // finalize + NVLink exchange + global merge of the row-sharded index
 // (finalize_exchange_kernel), the C-ABI entry points, and crag_knn_topk -- exact
@@ -49,19 +50,43 @@
 #include "knn_select.cuh"
 #include "knn_threshold.cuh"
 #include "pq_kernels.cuh"
+#include "binary.cuh"
 #include "workspace.cuh"
 
 namespace crag {
 
-// Dynamic shared memory of the scan, from a 1024-byte aligned base: the pipeline stages, the score tiles, the
-// selector (select_warps.cuh), then the mbarriers.
-template <int KLIST, int CAP, int STAGES>
+// Int8 variant of the flat top-k scan (I8Args, crag_search_topk_i8): the shard and the query block are int8 with one
+// fp32 scale per row / query (quant_kernels.cuh).  A 128-byte swizzle row holds 128 int8 instead of 64 bf16, so boxes,
+// stages, descriptors and score tiles keep their byte sizes; the warpgroup issues m64n32k32.s32.s8.s8 and its epilogue
+// writes S1 = float(acc) * (s_q * s_row) to the score tile, which the select warps rank as they rank bf16 scores.
+struct I8Args {
+  const float* row_scales;     // [n_rows], 0 on IVF padding rows
+  const float* query_scales;   // [nq] of this pass
+};
+// The int8 IVF scan (crag_ivf_search_i8): the select warps read the IvfArgs part, the wgmma warpgroup the scales.
+struct I8IvfArgs : IvfArgs, I8Args {};
+template <class Args> constexpr bool kI8Scan = std::is_base_of<I8Args, Args>::value;
+// One-bit variant (crag_search_topk_b1, binary.cuh): row_scales are the rows' alpha, the query block is int8 as for
+// I8Args, and so is the epilogue.  A stage holds one tile's code rows (128 rows x 128 bytes, 1024 columns at most) and
+// nothing else: the whole query block stays resident in shared memory, loaded once per launch, because streaming its
+// slice with every tile would cost about twice the code bytes in L2 reads.  The warpgroup widens its own A fragments
+// from the stage's bits and issues m64n32k32.s32.s8.s8 with A in registers.
+struct B1Args : I8Args {};
+template <class Args> constexpr bool kB1Scan = std::is_same<Args, B1Args>::value;
+
+// Dynamic shared memory of the scan, from a 1024-byte aligned base: the pipeline stages, (one-bit scan) the resident
+// query block, the score tiles, the selector (select_warps.cuh), then the mbarriers.
+template <int KLIST, int CAP, int STAGES, class Args>
 struct SearchLayout {
-  static constexpr size_t kTilesOff = size_t(STAGES) * kStageTotalBytes;
+  static constexpr bool kB1 = kB1Scan<Args>;
+  static constexpr size_t kStage = kB1 ? size_t(kStageBytes) : size_t(kStageTotalBytes);
+  static constexpr size_t kQueryOff = size_t(STAGES) * kStage;
+  static constexpr size_t kTilesOff = kQueryOff + (kB1 ? size_t(kB1QueryBytes) : 0);
   static constexpr size_t kSelectOff = kTilesOff + size_t(kAccStages) * kScoreTileBytes;
   static constexpr size_t kBarsOff = kSelectOff + SelectSmem<KLIST, CAP>::bytes();
+  static constexpr int kBars = 2 * STAGES + 2 * kAccStages + (kB1 ? 1 : 0);
   // + the alignment pad of the base and 16 bytes of slack past the mbarriers
-  __host__ __device__ static constexpr size_t smem_bytes() { return 1024 + kBarsOff + (2 * STAGES + 2 * kAccStages) * 8 + 16; }
+  __host__ __device__ static constexpr size_t smem_bytes() { return 1024 + kBarsOff + kBars * 8 + 16; }
 };
 
 // the 32 scores of row `row` of a score tile (layout: score_slot) -> r[q]
@@ -86,17 +111,51 @@ struct SmemScoreTiles {
   }
 };
 
-// Int8 variant of the flat top-k scan (I8Args, crag_search_topk_i8): the shard and the query block are int8 with one
-// fp32 scale per row / query (quant_kernels.cuh).  A 128-byte swizzle row holds 128 int8 instead of 64 bf16, so boxes,
-// stages, descriptors and score tiles keep their byte sizes; the warpgroup issues m64n32k32.s32.s8.s8 and its epilogue
-// writes S1 = float(acc) * (s_q * s_row) to the score tile, which the select warps rank as they rank bf16 scores.
-struct I8Args {
-  const float* row_scales;     // [n_rows], 0 on IVF padding rows
-  const float* query_scales;   // [nq] of this pass
-};
-// The int8 IVF scan (crag_ivf_search_i8): the select warps read the IvfArgs part, the wgmma warpgroup the scales.
-struct I8IvfArgs : IvfArgs, I8Args {};
-template <class Args> constexpr bool kI8Scan = std::is_base_of<I8Args, Args>::value;
+// The one-bit scan's MMA over one tile (B1Args): d[m] += A_m . Q^T over the num_kb 128-column chunks, A_m the +-1 rows
+// m * 64 .. m * 64 + 63 of the tile widened from the stage's bits (b1_a_fragment), Q the resident query block.  The
+// stage holds row r's 16-byte chunk kb at r * 128 + 16 (kb ^ r % 8) (TMA's 128-byte swizzle), so the 8 rows of one
+// load of a warp fall on distinct banks.  Chunks alternate between two register sets: the next chunk is widened while
+// the wgmma group of the current one runs, and only one group is in flight at a time, which is the pipelining ptxas
+// keeps without serialising register-A wgmmas (a second group in flight while A registers are written makes it
+// serialise them, C7513).
+__device__ __forceinline__ void b1_tile_mma(int32_t (&d)[2][16], const uint8_t* stage, int frag_row, int lane,
+                                            uint32_t q_addr, int num_kb) {
+  const int t = lane & 3;
+  const uint8_t* row0 = stage + frag_row * 128;   // this thread's rows frag_row, + 8, + 64, + 72
+  const int sw = frag_row & 7;                    // = r % 8 for all four
+  auto widen = [&](int kb, uint32_t (&a)[2][4][4]) {
+    const int off = (kb ^ sw) << 4;
+    const uint4 c[4] = {*reinterpret_cast<const uint4*>(row0 + off), *reinterpret_cast<const uint4*>(row0 + 8 * 128 + off),
+                        *reinterpret_cast<const uint4*>(row0 + 64 * 128 + off), *reinterpret_cast<const uint4*>(row0 + 72 * 128 + off)};
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+      const uint32_t lo[4] = {c[2 * m].x, c[2 * m].y, c[2 * m].z, c[2 * m].w};
+      const uint32_t hi[4] = {c[2 * m + 1].x, c[2 * m + 1].y, c[2 * m + 1].z, c[2 * m + 1].w};
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) b1_a_fragment(lo[ks], hi[ks], t, a[m][ks]);
+    }
+  };
+  auto mma = [&](int kb, uint32_t (&a)[2][4][4]) {
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {   // 32-column k-steps: 32 bytes of the query box's rows
+      const uint64_t db = wgmma_desc_sw128(q_addr + kb * kQBlockBytes + ks * 32);
+      wgmma_m64n32k32_s8_rs(d[0], a[0][ks], db, 1u);
+      wgmma_m64n32k32_s8_rs(d[1], a[1][ks], db, 1u);
+    }
+    wgmma_commit();
+  };
+  uint32_t a0[2][4][4], a1[2][4][4];
+  widen(0, a0);
+  for (int kb = 0; kb < num_kb; kb += 2) {
+    mma(kb, a0);
+    if (kb + 1 < num_kb) widen(kb + 1, a1);
+    wgmma_wait<0>();
+    if (kb + 1 < num_kb) mma(kb + 1, a1);
+    if (kb + 2 < num_kb) widen(kb + 2, a0);
+    wgmma_wait<0>();
+  }
+}
 
 template <int KLIST, int CAP, int STAGES, class Args>
 __global__ void __launch_bounds__(kSearchThreads, 1)
@@ -104,10 +163,11 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
                    int n_rows, int num_kb, int nq, int k, const uint64_t* __restrict__ after_keys,
                    uint64_t* __restrict__ pool, uint32_t perm_mul, int perm_shift, uint64_t* __restrict__ part_keys,
                    float* __restrict__ part_minmax, const Args args) {
-  constexpr bool IVF = kIvfScan<Args>, SCORES = kScoreScan<Args>, I8 = kI8Scan<Args>;
+  constexpr bool IVF = kIvfScan<Args>, SCORES = kScoreScan<Args>, I8 = kI8Scan<Args>, B1 = kB1Scan<Args>;
+  static_assert(!(B1 && (IVF || SCORES)), "the one-bit scan is a flat top-k scan");
   // elements per 128-byte swizzle row: the producer's column step per k-block
   constexpr int kBlockElems = I8 ? 128 : kBlockK;
-  using L = SearchLayout<KLIST, CAP, STAGES>;
+  using L = SearchLayout<KLIST, CAP, STAGES, Args>;
   static_assert(L::smem_bytes() <= 227 * 1024, "stages, score tiles and candidate lists exceed 227 KB of shared memory");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -119,6 +179,8 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
   uint64_t* bar_empty = bar_full + STAGES;
   uint64_t* bar_tfull = bar_empty + STAGES;            // [kAccStages]
   uint64_t* bar_tempty = bar_tfull + kAccStages;       // [kAccStages]
+  uint64_t* bar_q = bar_tempty + kAccStages;           // B1: the resident query block has landed
+  uint8_t* q_block = smem + L::kQueryOff;              // B1: num_kb boxes of 32 queries x 128 int8
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -137,6 +199,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
       mbar_init(&bar_tfull[a], 128); // every thread of the wgmma warpgroup, after its score stores
       mbar_init(&bar_tempty[a], 4);  // one arrive per select warp
     }
+    if constexpr (B1) mbar_init(bar_q, 1);
     fence_mbar_init();
   }
   sel.init(nq, after_keys);
@@ -150,9 +213,19 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
       const uint64_t pol = policy_evict_first();
       int stage = 0;
       uint32_t phase = 0;
+      if constexpr (B1) {   // the query block, once: num_kb boxes of 32 x 128 int8, 128-byte swizzled
+        mbar_arrive_expect_tx(bar_q, uint32_t(num_kb) * kQBlockBytes);
+        for (int kb = 0; kb < num_kb; ++kb) tma_load_2d(&tm_q, bar_q, q_block + kb * kQBlockBytes, kb * 128, 0);
+      }
       for (int j = blockIdx.x; j < num_tiles; j += gridDim.x) {
         const int tile = IVF ? j : order(j);
-        for (int kb = 0; kb < num_kb; ++kb) {
+        if constexpr (B1) {   // one box per tile: 128 code rows of 128 bytes (zero past dim8 / 8), 128-byte swizzled
+          mbar_wait(&bar_empty[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&bar_full[stage], kStageBytes);
+          tma_load_2d_hint(&tm_corpus, &bar_full[stage], stage_base + stage * L::kStage, 0, tile * kTileRows, pol);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        for (int kb = 0; kb < (B1 ? 0 : num_kb); ++kb) {
           mbar_wait(&bar_empty[stage], phase ^ 1);
           mbar_arrive_expect_tx(&bar_full[stage], kStageTotalBytes);
           int tile_row0;
@@ -186,6 +259,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
           q_scale[2 * j + c] = q < nq ? __ldg(&args.query_scales[q]) : 0.f;
         }
     }
+    if constexpr (B1) mbar_wait(bar_q, 0);
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       Acc d[2][16];
 #pragma unroll
@@ -203,7 +277,14 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
         }
       }
       int prev = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
+      if constexpr (B1) {
+        mbar_wait(&bar_full[stage], phase);
+        b1_tile_mma(d, stage_base + stage * L::kStage, frag_row, lane, smem_u32(q_block), num_kb);
+        __syncwarp();   // every lane has read its bits: the stage goes back to the producer
+        if (lane == 0) mbar_arrive(&bar_empty[stage]);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      for (int kb = 0; kb < (B1 ? 0 : num_kb); ++kb) {
         mbar_wait(&bar_full[stage], phase);
         const uint32_t a_addr = smem_u32(stage_base + stage * kStageTotalBytes);
         const uint32_t b_addr = a_addr + kStageBytes;
@@ -228,7 +309,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
       wgmma_wait<0>();
       wgmma_fence_regs(d[0]);
       wgmma_fence_regs(d[1]);
-      if (lane == 0) mbar_arrive(&bar_empty[prev]);
+      if (!B1 && lane == 0) mbar_arrive(&bar_empty[prev]);
       mbar_wait(&bar_tempty[acc], acc_phase ^ 1);
       float* st = score_tiles + acc * (kTileRows * kNQ);
 #pragma unroll
@@ -291,7 +372,7 @@ template <int KLIST, int CAP, int STAGES, class Args>
 int launch_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k, int grid,
                 const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift, uint64_t* part_keys,
                 float* part_minmax, const Args& args, cudaStream_t stream) {
-  constexpr size_t smem = SearchLayout<KLIST, CAP, STAGES>::smem_bytes();
+  constexpr size_t smem = SearchLayout<KLIST, CAP, STAGES, Args>::smem_bytes();
   auto kern = search_topk_kernel<KLIST, CAP, STAGES, Args>;
   static bool attr_set[64] = {};
   int dev = 0;
@@ -305,13 +386,19 @@ int launch_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_row
   return CRAG_OK;
 }
 
-// A top-k scan with the selector of k: 64-key lists and 6 stages up to k = 64, 128-key lists and 4 stages above.
+// A top-k scan with the selector of k: 64-key lists and 6 stages up to k = 64, 128-key lists and 4 stages above.  The
+// one-bit scan's stages are whole tiles and its query block takes 32 KB: 5 and 3 stages.
 template <class Args>
 int launch_topk_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_rows, int num_kb, int nq, int k,
                      int grid, const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift,
                      uint64_t* part_keys, float* part_minmax, const Args& args, cudaStream_t stream) {
-  if (k <= 64) return launch_scan<64, 64, 6>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
-  return launch_scan<128, 128, 4>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+  if constexpr (kB1Scan<Args>) {
+    if (k <= 64) return launch_scan<64, 64, 5>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+    return launch_scan<128, 128, 3>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+  } else {
+    if (k <= 64) return launch_scan<64, 64, 6>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+    return launch_scan<128, 128, 4>(tm_corpus, tm_q, n_rows, num_kb, nq, k, grid, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args, stream);
+  }
 }
 
 // The merge kernels' list size for k (32, 64 or 128), passed to `launch` as a std::integral_constant.
@@ -408,7 +495,9 @@ int scan_pass(const Operand& corpus, const Operand& queries, int k, const uint64
   int rc = make_tmap(&tm_corpus, corpus, kTileRows);
   if (rc == CRAG_OK) rc = make_tmap(&tm_q, queries, kNQ);
   if (rc != CRAG_OK) return rc;
-  return launch_topk_scan(tm_corpus, tm_q, int(corpus.rows), corpus.num_kb(), int(queries.rows), k, grid, after_keys, pool,
+  // k-blocks per pass over a row: 128-byte swizzle rows of a query (as many as a corpus row holds, except for one-bit
+  // codes, whose whole row is one box)
+  return launch_topk_scan(tm_corpus, tm_q, int(corpus.rows), queries.num_kb(), int(queries.rows), k, grid, after_keys, pool,
                           perm_multiplier(num_tiles >> kPermShift), kPermShift, plan.part_keys, plan.part_minmax, args, stream);
 }
 
@@ -819,6 +908,27 @@ extern "C" int crag_search_topk_i8(const void* corpus_i8, const float* row_scale
   if (rc != CRAG_OK) return rc;
   if (!query_scales || !out_ids || !out_scores || (n_rows > 0 && !row_scales)) return fail(CRAG_ERR_INVALID, "search_i8: null pointer");
   return topk_passes(c, q, k, row_offset, nullptr, I8Args{row_scales, query_scales}, out_ids, out_scores, out_minmax,
+                     nullptr, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------ one-bit shards (binary.cuh, quant_kernels.cuh)
+extern "C" int crag_search_topk_b1(const void* bits, const float* alpha, int64_t n_rows, int dim8, int64_t row_stride,
+                                   int64_t row_offset, const void* queries_i8, const float* query_scales, int nq, int k,
+                                   int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                                   size_t workspace_bytes, crag_stream_t stream) {
+  if (nq < 1 || k < 1 || k > 128) return fail(CRAG_ERR_INVALID, "search_b1: need nq >= 1 and 1 <= k <= 128 (nq=%d k=%d)", nq, k);
+  if (dim8 < 128 || dim8 > 1024 || dim8 % 128 != 0) return fail(CRAG_ERR_INVALID, "search_b1: dim8 must be a multiple of 128 in [128, 1024] (dim8=%d)", dim8);
+  if (n_rows < 0 || n_rows >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "search_b1: n_rows out of range (%lld)", (long long)n_rows);
+  if (row_stride < dim8 / 8 || row_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "search_b1: row_stride must be >= dim8 / 8 bytes and a multiple of 16 (row_stride=%lld)", (long long)row_stride);
+  if (n_rows > 0 && (!bits || !alpha)) return fail(CRAG_ERR_INVALID, "search_b1: null bits or alpha pointer");
+  if (reinterpret_cast<uintptr_t>(bits) & 15) return fail(CRAG_ERR_INVALID, "search_b1: bits must be 16-byte aligned");
+  if (!query_scales || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "search_b1: null query_scales or output pointer");
+  const Operand c{bits, n_rows, dim8 / 8, row_stride, kS8, "bits"}, q{queries_i8, nq, dim8, dim8, kS8, "queries_i8"};
+  const SearchPlan plan = plan_search(k, workspace);
+  int rc = check_operand("search_b1", q);
+  if (rc == CRAG_OK) rc = check_workspace("search_b1", workspace, workspace_bytes, plan.parts_bytes);
+  if (rc != CRAG_OK) return rc;
+  return topk_passes(c, q, k, row_offset, nullptr, B1Args{{alpha, query_scales}}, out_ids, out_scores, out_minmax,
                      nullptr, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
 }
 

@@ -42,18 +42,36 @@ def quantize_rows(rows: torch.Tensor, dim8: int, stream: Optional[torch.cuda.Str
 
 
 class QuantizedIndex:
-    """Frozen int8 snapshot of a DenseIndex's rows (rows added to the DenseIndex later are not seen)."""
+    """Frozen int8 snapshot of a DenseIndex's rows (rows added to the DenseIndex later are not seen).
 
-    def __init__(self, rows_bf16: torch.Tensor, rows_i8: torch.Tensor, scales: torch.Tensor, dim: int,
+    A subclass with another row code (binary.BinaryIndex) overrides _encode and _scan; the snapshot, the query checks
+    and the rescore are shared."""
+
+    def __init__(self, rows_bf16: torch.Tensor, codes: torch.Tensor, scales: torch.Tensor, dim: int,
                  device: torch.device, row_offset: int):
         self._rows = rows_bf16          # [n, dim_pad] bf16, on the device or in page-locked host memory
-        self._i8 = rows_i8              # [n, dim8] int8, device
+        self._codes = codes             # [n, dim8] int8 (the subclass's code rows), device
         self._scales = scales           # [n] fp32, device
         self.dim = dim
         self.dim_pad = rows_bf16.shape[1]
-        self.dim8 = rows_i8.shape[1]
+        self.dim8 = _dim8(self.dim_pad)
         self.device = device
         self.row_offset = row_offset
+
+    @staticmethod
+    def _encode(rows: torch.Tensor, dim8: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(code rows, per-row scales) of device bf16 rows."""
+        return quantize_rows(rows, dim8)
+
+    def _scan(self, q8: torch.Tensor, qs: torch.Tensor, candidates: int, c_ids: torch.Tensor, c_sc: torch.Tensor,
+              ws: torch.Tensor, st: torch.cuda.Stream) -> None:
+        """Stage 1: the top `candidates` rows of every query into (c_ids, c_sc)."""
+        n, nq = self.n_rows, q8.shape[0]
+        rc = _native.load().crag_search_topk_i8(self._codes.data_ptr() if n else 0, self._scales.data_ptr() if n else 0,
+                                                n, self.dim8, self.dim8, self.row_offset, q8.data_ptr(), qs.data_ptr(),
+                                                nq, candidates, c_ids.data_ptr(), c_sc.data_ptr(), 0, ws.data_ptr(),
+                                                ws.numel(), st.cuda_stream)
+        _native.check(rc, "crag_search_topk_i8")
 
     @classmethod
     def from_dense(cls, index: DenseIndex, rows: str = "device") -> "QuantizedIndex":
@@ -64,8 +82,8 @@ class QuantizedIndex:
         buf, n = index._snapshot()
         dev = index.device
         bf16 = buf[:n]
-        i8, scales = quantize_rows(bf16 if n else torch.zeros((0, index.dim_pad), dtype=torch.bfloat16, device=dev),
-                                   _dim8(index.dim_pad))
+        codes, scales = cls._encode(bf16 if n else torch.zeros((0, index.dim_pad), dtype=torch.bfloat16, device=dev),
+                                    _dim8(index.dim_pad))
         if rows == "host":
             host = torch.empty((n, index.dim_pad), dtype=torch.bfloat16, pin_memory=True)
             if n:
@@ -73,11 +91,11 @@ class QuantizedIndex:
             bf16 = host
         with torch.cuda.device(dev):
             torch.cuda.current_stream(dev).synchronize()   # the snapshot is complete when from_dense returns
-        return cls(bf16, i8, scales, index.dim, dev, index.row_offset)
+        return cls(bf16, codes, scales, index.dim, dev, index.row_offset)
 
     @property
     def n_rows(self) -> int:
-        return self._i8.shape[0]
+        return self._codes.shape[0]
 
     @property
     def rows_on_device(self) -> bool:
@@ -85,9 +103,9 @@ class QuantizedIndex:
 
     @property
     def device_bytes(self) -> int:
-        """Bytes this index holds in device memory: int8 rows, scales and, with rows="device", the bf16 rows (shared
+        """Bytes this index holds in device memory: code rows, scales and, with rows="device", the bf16 rows (shared
         with the DenseIndex it came from)."""
-        b = self._i8.numel() + 4 * self._scales.numel()
+        b = self._codes.numel() + 4 * self._scales.numel()
         if self._rows.is_cuda:
             b += 2 * self._rows.shape[0] * self._rows.stride(0) if self._rows.shape[0] else 0
         return b
@@ -99,7 +117,7 @@ class QuantizedIndex:
                       stream: Optional[torch.cuda.Stream] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Top k of a device bf16 [nq, dim_pad] query block: (ids int64 [nq, k], scores fp32 [nq, k]) on the device.
         Scores are the exact fp32 dots of the rescore (descending, ties by ascending id); -1 / -inf where fewer than
-        k rows exist.  candidates (default min(128, 4 k)) rows per query come from the int8 scan."""
+        k rows exist.  candidates (default min(128, 4 k)) rows per query come from the scan of the code rows."""
         if candidates is None:
             candidates = min(MAX_K, 4 * k)
         if not (1 <= k <= candidates <= MAX_K):
@@ -119,11 +137,7 @@ class QuantizedIndex:
                 c_sc = torch.empty((nq, candidates), dtype=torch.float32, device=dev)
                 ws_bytes = lib.crag_search_workspace_bytes(nq, candidates)
                 ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-                rc = lib.crag_search_topk_i8(self._i8.data_ptr() if n else 0, self._scales.data_ptr() if n else 0, n,
-                                             self.dim8, self.dim8, self.row_offset, q8.data_ptr(), qs.data_ptr(), nq,
-                                             candidates, c_ids.data_ptr(), c_sc.data_ptr(), 0, ws.data_ptr(), ws_bytes,
-                                             st.cuda_stream)
-                _native.check(rc, "crag_search_topk_i8")
+                self._scan(q8, qs, candidates, c_ids, c_sc, ws, st)
                 ids = torch.empty((nq, k), dtype=torch.int64, device=dev)
                 scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
                 rc = lib.crag_rescore_topk(self._rows.data_ptr() if n else 0, n, self.dim_pad,

@@ -142,6 +142,32 @@ CRAG_API int crag_rescore_topk(const void* rows_bf16, int64_t n_rows, int dim, i
                                const void* queries_bf16, int nq, const int64_t* cand_ids, int n_cand, int k,
                                int64_t* out_ids, float* out_scores, crag_stream_t stream);
 
+/* ------------------------------------------------------------------ one-bit shards
+ * A shard stored as sign codes with one fp32 scale per row: dim8 / 8 + 4 bytes per row (132 at dim 1024, against 2048
+ * for bf16 and 1028 for int8).  A search is crag_search_topk_b1 for k' candidates (k' <= 128) followed by
+ * crag_rescore_topk, as for int8 shards.  Semantics in DESIGN.md section 3f.
+ *
+ * crag_binarize_rows: bf16 [n_rows, dim] rows (device, row stride row_stride elements, 1 <= dim <= 1024) ->
+ *   out_bits  device uint8 [n_rows, out_stride], dim8 / 8 bytes written (dim8 = ceil(dim / 128) * 128): bit j of byte b
+ *             is 1 iff x_(8 b + j) > 0 (zero, -0 and padding columns give 0, which stands for -1); out_stride >= dim8 / 8
+ *             and a multiple of 16, 16-B aligned
+ *   out_alpha device fp32 [n_rows]: alpha = (sum |x_i|) / dim, the sum in crag_rescore_topk's pinned order; 0 for a
+ *             zero row.  Rows must be finite. */
+CRAG_API int crag_binarize_rows(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, void* out_bits,
+                                int64_t out_stride, float* out_alpha, crag_stream_t stream);
+/* crag_search_topk_b1: the top k (S1 descending, ties by ascending row) of
+ *   S1 = float(sum_i q^_i b_i) * (s_q * alpha_row),  b_i = +1 for a set bit, -1 for a clear one
+ *        (exact s32 sum; fp32 products rounded to nearest)
+ * over a one-bit shard (bits [n_rows, row_stride bytes] with dim8 / 8 code bytes per row, dim8 a multiple of 128 in
+ * [128, 1024]; row_stride >= dim8 / 8 and a multiple of 16, 16-B aligned; alpha fp32 [n_rows]) for queries_i8 int8
+ * [nq, dim8] dense with query_scales fp32 [nq], quantised by crag_quantize_rows_i8 (their zero padding cancels the -1
+ * padding bits).  Outputs, (min, max) (over the shard's S1), row_offset and workspace (crag_search_workspace_bytes(nq,
+ * k)) as crag_search_topk. */
+CRAG_API int crag_search_topk_b1(const void* bits, const float* alpha, int64_t n_rows, int dim8, int64_t row_stride,
+                                 int64_t row_offset, const void* queries_i8, const float* query_scales, int nq, int k,
+                                 int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                                 size_t workspace_bytes, crag_stream_t stream);
+
 /* Exact top-k for large k and/or many queries: per chunk of queries one wgmma GEMM writes the fp32 score block
  * [q_chunk, round_up(n_rows, 4)] into the workspace, then one CTA per query radix-selects its k best.
  * Same argument rules and the same output contract as crag_search_topk (score desc, ties by ascending row, -1/-inf

@@ -101,7 +101,7 @@ def main():
                                                    ws.numel(), st), "crag_search_topk")
 
             def i8():
-                _native.check(lib.crag_search_topk_i8(qd._i8.data_ptr(), qd._scales.data_ptr(), n, qd.dim8, qd.dim8, 0,
+                _native.check(lib.crag_search_topk_i8(qd._codes.data_ptr(), qd._scales.data_ptr(), n, qd.dim8, qd.dim8, 0,
                                                       q8.data_ptr(), qs.data_ptr(), a.nq, cand, ids.data_ptr(),
                                                       sc.data_ptr(), mm.data_ptr(), ws.data_ptr(), ws.numel(), st),
                               "crag_search_topk_i8")
