@@ -14,28 +14,13 @@ from typing import Optional, Tuple
 import torch
 
 from . import _native
-from .quantized import QuantizedIndex
+from .quantized import QuantizedIndex, _dim8, _encode_rows
 
 
 def binarize_rows(rows: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """crag_binarize_rows of a device bf16 [n, dim] tensor (unit inner stride): (uint8 codes [n, dim8 / 8], fp32 alpha
     [n]), dim8 = dim rounded up to a multiple of 128."""
-    if rows.dtype != torch.bfloat16 or rows.dim() != 2 or not rows.is_cuda or (rows.shape[0] > 1 and rows.stride(1) != 1):
-        raise ValueError("binarize_rows expects a CUDA bf16 [n, dim] tensor with unit inner stride")
-    n, dim = rows.shape
-    width = (dim + 127) // 128 * 16
-    dev = rows.device
-    lib = _native.load()
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        with torch.cuda.stream(st):
-            bits = torch.empty((n, width), dtype=torch.uint8, device=dev)
-            alpha = torch.empty((n,), dtype=torch.float32, device=dev)
-            rc = lib.crag_binarize_rows(rows.data_ptr() if n else 0, n, dim, rows.stride(0) if n else dim,
-                                        bits.data_ptr() if n else 0, width, alpha.data_ptr() if n else 0,
-                                        st.cuda_stream)
-            _native.check(rc, "crag_binarize_rows")
-    return bits, alpha
+    return _encode_rows("binarize_rows", "crag_binarize_rows", rows, lambda dim: _dim8(dim) // 8, torch.uint8, stream)
 
 
 class BinaryIndex(QuantizedIndex):

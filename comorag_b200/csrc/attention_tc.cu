@@ -194,15 +194,8 @@ int launch_attention_tc(const void* qkv, const int32_t* cu_seqlens, int n_seqs, 
   if (rc != CRAG_OK) return rc;
   const dim3 grid((max_len + kAttBM - 1) / kAttBM, heads, n_seqs);
   const float scale_log2e = 1.4426950408889634f / sqrtf(float(kAttDH));
-  {  // once per device, not per launch
-    static bool done[64] = {false};
-    int dev = 0;
-    CRAG_CUDA_OK(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !done[dev]) {
-      CRAG_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kAttSmemBytes)));
-      if (dev >= 0 && dev < 64) done[dev] = true;
-    }
-  }
+  rc = allow_dynamic_smem<attention_tc_kernel>(kAttSmemBytes);
+  if (rc != CRAG_OK) return rc;
   attention_tc_kernel<<<grid, kAttThreads, kAttSmemBytes, stream>>>(tm_q, tm_kv, cu_seqlens, H, scale_log2e,
                                                                     static_cast<__nv_bfloat16*>(ctx));
   CRAG_CUDA_OK(cudaGetLastError());

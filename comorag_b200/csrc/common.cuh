@@ -1,8 +1,9 @@
 // Host-side helpers shared by the translation units of libcomorag_b200:
 // error reporting for the C ABI, TMA tensor-map construction (driver entry
-// point fetched through the runtime, so the library links only cudart), and
-// device queries.
+// point fetched through the runtime, so the library links only cudart),
+// device queries and the dynamic shared-memory opt-in of a kernel.
 #pragma once
+#include <atomic>
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -34,6 +35,21 @@ int make_tmap_u8_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t 
                     uint32_t box_rows, uint32_t box_cols = 128);
 
 int sm_count();
+
+// Raise Kernel's dynamic shared-memory limit to `bytes` once per device, not per launch.  The flags belong to the kernel
+// itself (two instantiations of one kernel template do not share them) and are safe under concurrent host threads; a
+// race at most repeats the idempotent attribute call.
+template <auto Kernel>
+int allow_dynamic_smem(size_t bytes) {
+  static std::atomic<bool> done[64];
+  int dev = 0;
+  CRAG_CUDA_OK(cudaGetDevice(&dev));
+  const bool tracked = dev >= 0 && dev < 64;
+  if (tracked && done[dev].load(std::memory_order_acquire)) return CRAG_OK;
+  CRAG_CUDA_OK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes)));
+  if (tracked) done[dev].store(true, std::memory_order_release);
+  return CRAG_OK;
+}
 
 // A workspace argument (workspace.cuh): CRAG_ERR_INVALID when null or not kWsAlign-aligned, CRAG_ERR_WORKSPACE when
 // `bytes` < `need`; `who` heads the message.

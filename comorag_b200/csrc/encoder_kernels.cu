@@ -305,8 +305,10 @@ int launch_pool_normalize(const void* hidden, const int32_t* cu_seqlens, int n_s
                           float* out_f32, void* out_bf16, int64_t out_bf16_stride, cudaStream_t stream) {
   if (n_seqs <= 0) return CRAG_OK;
   if (H > 2048) return fail(CRAG_ERR_UNSUPPORTED, "hidden size %d > 2048 not supported", H);
-  const size_t smem = (size_t(kPoolGroups) * H + 4) * sizeof(float);
-  if (smem > 48 * 1024) CRAG_CUDA_OK(cudaFuncSetAttribute(pool_normalize_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  const auto smem_bytes = [](int h) { return (size_t(kPoolGroups) * h + 4) * sizeof(float); };
+  const int rc = allow_dynamic_smem<pool_normalize_kernel>(smem_bytes(2048));
+  if (rc != CRAG_OK) return rc;
+  const size_t smem = smem_bytes(H);
   pool_normalize_kernel<<<n_seqs, 128 * kPoolGroups, smem, stream>>>(static_cast<const __nv_bfloat16*>(hidden), cu_seqlens, H,
                                                                      normalize, out_f32, static_cast<__nv_bfloat16*>(out_bf16),
                                                                      out_bf16_stride);

@@ -191,19 +191,11 @@ template <int EPI>
 static int launch_gemm_t(const CUtensorMap& tm_a, const CUtensorMap& tm_b, int M, int N, int K, const float* bias,
                          const __nv_bfloat16* residual, int64_t ldr, __nv_bfloat16* out, int64_t ldo,
                          cudaStream_t stream) {
-  auto kern = gemm_bf16_kernel<EPI>;
-  {  // once per kernel and device, not per launch
-    static bool done[64] = {false};
-    int dev = 0;
-    CRAG_CUDA_OK(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !done[dev]) {
-      CRAG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(GemmLayout::smem_bytes())));
-      if (dev >= 0 && dev < 64) done[dev] = true;
-    }
-  }
+  const int rc = allow_dynamic_smem<gemm_bf16_kernel<EPI>>(GemmLayout::smem_bytes());
+  if (rc != CRAG_OK) return rc;
   const unsigned n_blocks = (N + kGemmBN - 1) / kGemmBN, m_blocks = (M + kGemmBM - 1) / kGemmBM;
   const dim3 grid = EPI == GEMM_EPI_SCORES_F32 ? dim3(m_blocks * n_blocks) : dim3(n_blocks, m_blocks);
-  kern<<<grid, kGemmThreads, GemmLayout::smem_bytes(), stream>>>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo);
+  gemm_bf16_kernel<EPI><<<grid, kGemmThreads, GemmLayout::smem_bytes(), stream>>>(tm_a, tm_b, M, N, K, bias, residual, ldr, out, ldo);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }

@@ -373,15 +373,9 @@ int launch_scan(const CUtensorMap& tm_corpus, const CUtensorMap& tm_q, int n_row
                 const uint64_t* after_keys, uint64_t* pool, uint32_t perm_mul, int perm_shift, uint64_t* part_keys,
                 float* part_minmax, const Args& args, cudaStream_t stream) {
   constexpr size_t smem = SearchLayout<KLIST, CAP, STAGES, Args>::smem_bytes();
-  auto kern = search_topk_kernel<KLIST, CAP, STAGES, Args>;
-  static bool attr_set[64] = {};
-  int dev = 0;
-  CRAG_CUDA_OK(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-    CRAG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-    if (dev >= 0 && dev < 64) attr_set[dev] = true;
-  }
-  kern<<<grid, kSearchThreads, smem, stream>>>(tm_corpus, tm_q, n_rows, num_kb, nq, k, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args);
+  const int rc = allow_dynamic_smem<search_topk_kernel<KLIST, CAP, STAGES, Args>>(smem);
+  if (rc != CRAG_OK) return rc;
+  search_topk_kernel<KLIST, CAP, STAGES, Args><<<grid, kSearchThreads, smem, stream>>>(tm_corpus, tm_q, n_rows, num_kb, nq, k, after_keys, pool, perm_mul, perm_shift, part_keys, part_minmax, args);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }
@@ -416,7 +410,9 @@ Args pass_args(Args args, int q0) {
   return args;
 }
 
-// A scan operand: `rows` rows of `width` elements, `stride` elements apart; `name` heads its error messages.
+// A scan operand: `rows` rows of `width` elements, `stride` elements apart; `name` heads its error messages.  `bits`
+// marks a one-bit shard's sign-bit rows: dim8 / 8 bytes each, read as one zero-filled 128-byte box per row, so their
+// width has no rule of its own and follows from the queries' dim8.
 enum Elem { kS8 = 1, kBf16 = 2 };   // bytes per element
 struct Operand {
   const void* ptr;
@@ -425,27 +421,30 @@ struct Operand {
   int64_t stride;
   Elem elem;
   const char* name;
-  Operand rows_from(int64_t r0, int64_t n) const { return {static_cast<const uint8_t*>(ptr) + r0 * stride * elem, n, width, stride, elem, name}; }
+  bool bits = false;
+  Operand rows_from(int64_t r0, int64_t n) const { return {static_cast<const uint8_t*>(ptr) + r0 * stride * elem, n, width, stride, elem, name, bits}; }
   int num_kb() const { return width * elem / 128; }   // 128-byte swizzle rows per row
 };
 
 // The scan's rules for an operand, in bytes: 1 to 1024 elements per row in whole 128-byte swizzle rows (bf16 dim % 64,
-// int8 dim % 128), a row stride of whole 16 bytes, a 16-byte aligned base and row indices that fit an int.
+// int8 dim8 % 128), a row stride of whole 16 bytes, a 16-byte aligned base and row indices that fit an int.
 int check_operand(const char* who, const Operand& op) {
-  if (op.width < 1 || op.width > 1024 || op.width * op.elem % 128 != 0) return fail(CRAG_ERR_INVALID, "%s: %s dim must be a multiple of %d in [%d, 1024] (dim=%d)", who, op.name, 128 / op.elem, 128 / op.elem, op.width);
+  const char* dim = op.elem == kS8 ? "dim8" : "dim";
+  if (!op.bits && (op.width < 1 || op.width > 1024 || op.width * op.elem % 128 != 0)) return fail(CRAG_ERR_INVALID, "%s: %s %s must be a multiple of %d in [%d, 1024] (%s=%d)", who, op.name, dim, 128 / op.elem, 128 / op.elem, dim, op.width);
   if (op.rows < 0 || op.rows >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "%s: %s n_rows out of range (%lld)", who, op.name, (long long)op.rows);
-  if (op.stride < op.width || op.stride * op.elem % 16 != 0) return fail(CRAG_ERR_INVALID, "%s: %s row stride must be >= dim and a multiple of %d", who, op.name, 16 / op.elem);
+  if (op.stride < op.width || op.stride * op.elem % 16 != 0) return fail(CRAG_ERR_INVALID, "%s: %s row_stride must be >= %s and a multiple of %d", who, op.name, op.bits ? "dim8 / 8 bytes" : dim, 16 / op.elem);
   if (op.rows > 0 && !op.ptr) return fail(CRAG_ERR_INVALID, "%s: null %s pointer", who, op.name);
   if (reinterpret_cast<uintptr_t>(op.ptr) & 15) return fail(CRAG_ERR_INVALID, "%s: %s must be 16-byte aligned", who, op.name);
   return CRAG_OK;
 }
 
-// nq and k, the shard and query operands of a scan, and a 256-byte aligned workspace of at least `need` bytes
+// nq and k, the query and shard operands of a scan, and a 256-byte aligned workspace of at least `need` bytes.  The
+// queries come first: their width rule is the shard's too, and the only one a one-bit shard has.
 int check_scan_args(const char* who, int nq, int k, int k_max, const Operand& corpus, const Operand& queries,
                     const void* workspace, size_t workspace_bytes, size_t need) {
   if (nq < 1 || k < 1 || k > k_max) return fail(CRAG_ERR_INVALID, "%s: need nq >= 1 and 1 <= k <= %d (nq=%d k=%d)", who, k_max, nq, k);
-  int rc = check_operand(who, corpus);
-  if (rc == CRAG_OK) rc = check_operand(who, queries);
+  int rc = check_operand(who, queries);
+  if (rc == CRAG_OK) rc = check_operand(who, corpus);
   if (rc != CRAG_OK) return rc;
   return check_workspace(who, workspace, workspace_bytes, need);
 }
@@ -588,47 +587,38 @@ int check_ivf_args(const char* who, const IvfLists& l, int64_t n_rows_padded, co
   return CRAG_OK;
 }
 
-// crag_ivf_search_i8's exact rescore: bf16 residuals (device address) and queries, and the candidates' workspace buffers
+// the exact rescore of crag_ivf_search_i8 and crag_ivf_search_pq: bf16 residuals (device address) and queries, and
+// the candidates' workspace buffers
 struct IvfRescore {
   Operand rows, queries;
   int64_t* cand_ids;
   float* cand_scores;
 };
 
-// Every 32-query pass of an IVF search over the residuals `res`: the plan of the probed tiles, the scan for n_scan keys
-// per query, the merge of its partials, then the map of stored positions to original ids.  With `rescore` the merge
-// writes n_scan candidates, which the exact rescore (quant.cu) turns into the k results, with the plan's coarse terms.
-template <class Args>
-int ivf_passes(const Operand& res, const Operand& queries, Args args, const IvfLists& l, int n_scan, int k,
-               const IvfRescore* rescore, int64_t* out_ids, float* out_scores, float* out_minmax, const IvfPlan& ip,
-               cudaStream_t stream) {
+// Every 32-query pass of an IVF search: the plan of the probed tiles, stage 1 for n_scan keys per query, the merge of
+// its partials, then the map of stored positions to original ids.  `stage1(q0, nqc, parts)` launches stage 1 for
+// queries q0 .. q0 + nqc - 1 and sets `parts` to the number of partial lists it wrote.  With `rescore` the merge writes
+// n_scan candidates, which the exact rescore (quant.cu) turns into the k results, with the plan's coarse terms.
+template <class Stage1>
+int ivf_passes(int nq, const IvfLists& l, int n_scan, int k, const IvfRescore* rescore, int64_t* out_ids,
+               float* out_scores, float* out_minmax, const IvfPlan& ip, cudaStream_t stream, Stage1 stage1) {
   const SearchPlan& sp = ip.scan;
-  static_cast<IvfArgs&>(args) = IvfArgs{ip.work, ip.n_work, ip.list_mask, ip.coarse};
-  CUtensorMap tm_res;
-  int rc = make_tmap(&tm_res, res, kTileRows);
-  if (rc != CRAG_OK) return rc;
-  const int nq = int(queries.rows);
   for (int q0 = 0; q0 < nq; q0 += kNQ) {
     const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
-    CUtensorMap tm_q;
-    rc = make_tmap(&tm_q, queries.rows_from(q0, nqc), kNQ);
-    if (rc != CRAG_OK) return rc;
     ivf_plan_kernel<<<1, 1024, 0, stream>>>(l.probed_ids + size_t(q0) * l.nprobe, l.probed_scores + size_t(q0) * l.nprobe, nqc,
                                             l.nprobe, l.nlist, l.tile_start, l.rows, ip.list_mask, ip.coarse, ip.work,
                                             ip.n_work);
     CRAG_CUDA_OK(cudaGetLastError());
-    // every CTA of the grid publishes a (possibly empty) partial list, so the merge always reads sp.grid parts
-    if (sp.pool) CRAG_CUDA_OK(cudaMemsetAsync(sp.pool, 0, sp.pool_bytes, stream));
-    rc = launch_topk_scan(tm_res, tm_q, int(res.rows), res.num_kb(), nqc, n_scan, sp.grid, nullptr, sp.pool, 0u, 0,
-                          sp.part_keys, sp.part_minmax, pass_args(args, q0), stream);
+    int parts = 0;
+    int rc = stage1(q0, nqc, parts);
     if (rc != CRAG_OK) return rc;
     int64_t* ids = out_ids + size_t(q0) * k;
     float* scores = out_scores + size_t(q0) * k;
     float* minmax = out_minmax ? out_minmax + size_t(q0) * 2 : nullptr;
     if (!rescore) {
-      rc = finalize_parts(sp.grid, nqc, k, 0, ids, scores, minmax, nullptr, sp, stream);
+      rc = finalize_parts(parts, nqc, k, 0, ids, scores, minmax, nullptr, sp, stream);
     } else {
-      rc = finalize_parts(sp.grid, nqc, n_scan, 0, rescore->cand_ids, rescore->cand_scores, minmax, nullptr, sp, stream);
+      rc = finalize_parts(parts, nqc, n_scan, 0, rescore->cand_ids, rescore->cand_scores, minmax, nullptr, sp, stream);
       if (rc == CRAG_OK)
         rc = launch_ivf_rescore(rescore->rows.ptr, rescore->rows.rows, rescore->rows.width, rescore->rows.stride,
                                 rescore->queries.rows_from(q0, nqc).ptr, nqc, rescore->cand_ids, n_scan, k, l.tile_start,
@@ -639,6 +629,51 @@ int ivf_passes(const Operand& res, const Operand& queries, Args args, const IvfL
     CRAG_CUDA_OK(cudaGetLastError());
   }
   return CRAG_OK;
+}
+
+// The IVF passes whose stage 1 is the scan of the probed tiles of the residuals `res` (bf16 or int8, as Args says).
+// Every CTA of the grid publishes a (possibly empty) partial list, so the merge reads sp.grid parts.
+template <class Args>
+int ivf_scan_passes(const Operand& res, const Operand& queries, Args args, const IvfLists& l, int n_scan, int k,
+                    const IvfRescore* rescore, int64_t* out_ids, float* out_scores, float* out_minmax,
+                    const IvfPlan& ip, cudaStream_t stream) {
+  const SearchPlan& sp = ip.scan;
+  static_cast<IvfArgs&>(args) = IvfArgs{ip.work, ip.n_work, ip.list_mask, ip.coarse};
+  CUtensorMap tm_res;
+  int rc = make_tmap(&tm_res, res, kTileRows);
+  if (rc != CRAG_OK) return rc;
+  return ivf_passes(int(queries.rows), l, n_scan, k, rescore, out_ids, out_scores, out_minmax, ip, stream,
+                    [&](int q0, int nqc, int& parts) {
+                      CUtensorMap tm_q;
+                      const int rc = make_tmap(&tm_q, queries.rows_from(q0, nqc), kNQ);
+                      if (rc != CRAG_OK) return rc;
+                      if (sp.pool) CRAG_CUDA_OK(cudaMemsetAsync(sp.pool, 0, sp.pool_bytes, stream));
+                      parts = sp.grid;
+                      return launch_topk_scan(tm_res, tm_q, int(res.rows), res.num_kb(), nqc, n_scan, sp.grid, nullptr,
+                                              sp.pool, 0u, 0, sp.part_keys, sp.part_minmax, pass_args(args, q0), stream);
+                    });
+}
+
+// The argument rules of the rescored IVF searches (crag_ivf_search_i8, crag_ivf_search_pq): the lists, probes and
+// outputs, nq >= 1 and 1 <= k <= n_cand <= 128, then the entry's own rules (`entry_check()`), the bf16 residuals and
+// queries of the rescore, and a workspace of `need` bytes.  Then points r.rows at the device address of the bf16
+// residuals, which may be page-locked host memory (pageable memory is refused before any launch), and r's candidates
+// at `cand`'s buffers.
+template <class EntryCheck>
+int check_rescored_ivf(const char* who, const IvfLists& l, int64_t n_rows_padded, int nq, int n_cand, int k,
+                       const int64_t* out_ids, const float* out_scores, IvfRescore& r, const IvfI8Plan& cand,
+                       const void* workspace, size_t workspace_bytes, size_t need, EntryCheck entry_check) {
+  int rc = check_ivf_args(who, l, n_rows_padded, out_ids, out_scores);
+  if (rc != CRAG_OK) return rc;
+  if (nq < 1 || k < 1 || n_cand < k || n_cand > 128) return fail(CRAG_ERR_INVALID, "%s: need nq >= 1 and 1 <= k <= n_cand <= 128 (nq=%d k=%d n_cand=%d)", who, nq, k, n_cand);
+  rc = entry_check();
+  if (rc == CRAG_OK) rc = check_operand(who, r.rows);
+  if (rc == CRAG_OK) rc = check_operand(who, r.queries);
+  if (rc == CRAG_OK) rc = check_workspace(who, workspace, workspace_bytes, need);
+  if (rc == CRAG_OK) rc = device_readable(r.rows.ptr, &r.rows.ptr, who);
+  r.cand_ids = cand.cand_ids;
+  r.cand_scores = cand.cand_scores;
+  return rc;
 }
 
 }  // namespace
@@ -662,8 +697,8 @@ extern "C" int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int
   const IvfPlan ip = plan_ivf(k >= 1 && k <= 128 ? k : 1, nlist, total_tiles, workspace);
   rc = check_scan_args("ivf", nq, k, 128, res, q, workspace, workspace_bytes, ip.total);
   if (rc != CRAG_OK) return rc;
-  return ivf_passes(res, q, IvfArgs{}, lists, k, k, nullptr, out_ids, out_scores, out_minmax, ip,
-                    static_cast<cudaStream_t>(stream));
+  return ivf_scan_passes(res, q, IvfArgs{}, lists, k, k, nullptr, out_ids, out_scores, out_minmax, ip,
+                         static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------ IVF over int8 residuals (ivf_passes with a rescore)
@@ -684,23 +719,18 @@ extern "C" int crag_ivf_search_i8(const void* residuals_i8, const float* row_sca
   IvfRescore rescore{{residuals_bf16, n_rows_padded, dim, row_stride, kBf16, "residuals_bf16"},
                      {queries_bf16, nq, dim, dim, kBf16, "queries_bf16"}, nullptr, nullptr};
   const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
-  int rc = check_ivf_args("ivf_i8", lists, n_rows_padded, out_ids, out_scores);
-  if (rc != CRAG_OK) return rc;
-  if (nq < 1 || k < 1 || n_cand < k || n_cand > 128) return fail(CRAG_ERR_INVALID, "ivf_i8: need nq >= 1 and 1 <= k <= n_cand <= 128 (nq=%d k=%d n_cand=%d)", nq, k, n_cand);
-  if (dim8 != (dim + 127) / 128 * 128) return fail(CRAG_ERR_INVALID, "ivf_i8: dim8 must be dim rounded up to a multiple of 128 (dim=%d dim8=%d)", dim, dim8);
   const IvfI8Plan plan = plan_ivf_i8(nlist, total_tiles, n_cand, workspace);
-  rc = check_scan_args("ivf_i8", nq, n_cand, 128, res, q, workspace, workspace_bytes, plan.total);
-  if (rc == CRAG_OK) rc = check_operand("ivf_i8", rescore.rows);
-  if (rc == CRAG_OK) rc = check_operand("ivf_i8", rescore.queries);
+  const int rc = check_rescored_ivf("ivf_i8", lists, n_rows_padded, nq, n_cand, k, out_ids, out_scores, rescore, plan,
+                                    workspace, workspace_bytes, plan.total, [&] {
+    if (dim8 != (dim + 127) / 128 * 128) return fail(CRAG_ERR_INVALID, "ivf_i8: dim8 must be dim rounded up to a multiple of 128 (dim=%d dim8=%d)", dim, dim8);
+    int rc = check_operand("ivf_i8", res);
+    if (rc == CRAG_OK) rc = check_operand("ivf_i8", q);
+    if (rc == CRAG_OK && (!row_scales || !query_scales)) rc = fail(CRAG_ERR_INVALID, "ivf_i8: null pointer");
+    return rc;
+  });
   if (rc != CRAG_OK) return rc;
-  if (!row_scales || !query_scales) return fail(CRAG_ERR_INVALID, "ivf_i8: null pointer");
-  // the bf16 residuals may be page-locked host memory: refused before any launch if pageable
-  rc = device_readable(residuals_bf16, &rescore.rows.ptr, "ivf_i8");
-  if (rc != CRAG_OK) return rc;
-  rescore.cand_ids = plan.cand_ids;
-  rescore.cand_scores = plan.cand_scores;
-  return ivf_passes(res, q, I8IvfArgs{{}, {row_scales, query_scales}}, lists, n_cand, k, &rescore, out_ids, out_scores, out_minmax, plan.ivf,
-                    static_cast<cudaStream_t>(stream));
+  return ivf_scan_passes(res, q, I8IvfArgs{{}, {row_scales, query_scales}}, lists, n_cand, k, &rescore, out_ids, out_scores,
+                         out_minmax, plan.ivf, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------ IVF over product-quantized residuals (pq_kernels.cuh)
@@ -728,63 +758,6 @@ int check_pq_shape(const char* who, int dim, int m) {
   return CRAG_OK;
 }
 
-// The dynamic shared-memory limit of a kernel is raised once per device, to what its largest shape needs.
-template <class Kernel>
-int allow_smem(Kernel kern, size_t bytes, bool (&done)[64]) {
-  int dev = 0;
-  CRAG_CUDA_OK(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64 || !done[dev]) {
-    CRAG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes)));
-    if (dev >= 0 && dev < 64) done[dev] = true;
-  }
-  return CRAG_OK;
-}
-
-// Every 32-query pass of a PQ IVF search: the plan, the queries' tables, the PQ scan for n_cand candidates, the merge
-// of its partials, the exact rescore of the candidates and the map of stored positions to original ids.
-int ivf_pq_passes(const uint8_t* codes, int64_t code_stride, int m, const float* codebooks, const IvfLists& l,
-                  int n_cand, int k, const IvfRescore& rescore, int64_t* out_ids, float* out_scores, float* out_minmax,
-                  const IvfPqPlan& pp, cudaStream_t stream) {
-  const IvfPlan& ip = pp.cand.ivf;
-  const SearchPlan& sp = ip.scan;
-  const IvfArgs args{ip.work, ip.n_work, ip.list_mask, ip.coarse};
-  const int nq = int(rescore.queries.rows), dim = rescore.queries.width;
-  for (int q0 = 0; q0 < nq; q0 += kNQ) {
-    const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
-    ivf_plan_kernel<<<1, 1024, 0, stream>>>(l.probed_ids + size_t(q0) * l.nprobe, l.probed_scores + size_t(q0) * l.nprobe, nqc,
-                                            l.nprobe, l.nlist, l.tile_start, l.rows, ip.list_mask, ip.coarse, ip.work,
-                                            ip.n_work);
-    CRAG_CUDA_OK(cudaGetLastError());
-    const void* qp = rescore.queries.rows_from(q0, nqc).ptr;
-    pq_table_kernel<<<unsigned(nqc * m), kPqTableThreads, 0, stream>>>(static_cast<const uint16_t*>(qp), dim, codebooks, m, pp.lut);
-    CRAG_CUDA_OK(cudaGetLastError());
-    // about two CTAs per SM in all; every (slice, query) CTA writes its part, so the merge reads `slices` parts
-    const int slices = std::min(sp.grid, std::max(1, (2 * sp.grid + nqc - 1) / nqc));
-    int rc = CRAG_OK;
-    with_merge_tier(n_cand, [&](auto tier) {
-      constexpr int T = decltype(tier)::value;
-      static bool attr_set[64] = {};
-      rc = allow_smem(pq_scan_kernel<T>, PqScanSmem<T>::bytes(kPqMaxM), attr_set);
-      if (rc != CRAG_OK) return;
-      pq_scan_kernel<T><<<unsigned(nqc * slices), kPqThreads, PqScanSmem<T>::bytes(m), stream>>>(
-          codes, code_stride, m, pp.lut, slices, n_cand, args, sp.part_keys, sp.part_minmax);
-    });
-    if (rc != CRAG_OK) return rc;
-    CRAG_CUDA_OK(cudaGetLastError());
-    float* minmax = out_minmax ? out_minmax + size_t(q0) * 2 : nullptr;
-    int64_t* ids = out_ids + size_t(q0) * k;
-    rc = finalize_parts(slices, nqc, n_cand, 0, pp.cand.cand_ids, pp.cand.cand_scores, minmax, nullptr, sp, stream);
-    if (rc == CRAG_OK)
-      rc = launch_ivf_rescore(rescore.rows.ptr, rescore.rows.rows, rescore.rows.width, rescore.rows.stride, qp, nqc,
-                              pp.cand.cand_ids, n_cand, k, l.tile_start, l.nlist, ip.coarse, ids,
-                              out_scores + size_t(q0) * k, stream);
-    if (rc != CRAG_OK) return rc;
-    ivf_map_ids_kernel<<<(nqc * k + 255) / 256, 256, 0, stream>>>(ids, nqc * k, l.row_ids);
-    CRAG_CUDA_OK(cudaGetLastError());
-  }
-  return CRAG_OK;
-}
-
 }  // namespace
 }  // namespace crag
 
@@ -803,24 +776,40 @@ extern "C" int crag_ivf_search_pq(const void* codes, int m, int64_t code_stride,
   IvfRescore rescore{{residuals_bf16, n_rows_padded, dim, row_stride, kBf16, "residuals_bf16"},
                      {queries_bf16, nq, dim, dim, kBf16, "queries_bf16"}, nullptr, nullptr};
   const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
-  int rc = check_ivf_args("ivf_pq", lists, n_rows_padded, out_ids, out_scores);
-  if (rc != CRAG_OK) return rc;
-  if (nq < 1 || k < 1 || n_cand < k || n_cand > 128) return fail(CRAG_ERR_INVALID, "ivf_pq: need nq >= 1 and 1 <= k <= n_cand <= 128 (nq=%d k=%d n_cand=%d)", nq, k, n_cand);
-  rc = check_pq_shape("ivf_pq", dim, m);
-  if (rc != CRAG_OK) return rc;
-  if (code_stride < pq_code_stride(m) || code_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "ivf_pq: code_stride must be a multiple of 16 and >= %d (code_stride=%lld)", pq_code_stride(m), (long long)code_stride);
-  if (!codes || !codebooks) return fail(CRAG_ERR_INVALID, "ivf_pq: null codes or codebooks pointer");
-  if ((reinterpret_cast<uintptr_t>(codes) | reinterpret_cast<uintptr_t>(codebooks)) & 15) return fail(CRAG_ERR_INVALID, "ivf_pq: codes and codebooks must be 16-byte aligned");
-  rc = check_operand("ivf_pq", rescore.rows);
-  if (rc == CRAG_OK) rc = check_operand("ivf_pq", rescore.queries);
   const IvfPqPlan plan = plan_ivf_pq(nlist, total_tiles, n_cand, m, workspace);
-  if (rc == CRAG_OK) rc = check_workspace("ivf_pq", workspace, workspace_bytes, plan.total);
+  const int rc = check_rescored_ivf("ivf_pq", lists, n_rows_padded, nq, n_cand, k, out_ids, out_scores, rescore, plan.cand,
+                                    workspace, workspace_bytes, plan.total, [&] {
+    const int rc = check_pq_shape("ivf_pq", dim, m);
+    if (rc != CRAG_OK) return rc;
+    if (code_stride < pq_code_stride(m) || code_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "ivf_pq: code_stride must be a multiple of 16 and >= %d (code_stride=%lld)", pq_code_stride(m), (long long)code_stride);
+    if (!codes || !codebooks) return fail(CRAG_ERR_INVALID, "ivf_pq: null codes or codebooks pointer");
+    if ((reinterpret_cast<uintptr_t>(codes) | reinterpret_cast<uintptr_t>(codebooks)) & 15) return fail(CRAG_ERR_INVALID, "ivf_pq: codes and codebooks must be 16-byte aligned");
+    return CRAG_OK;
+  });
   if (rc != CRAG_OK) return rc;
-  // the bf16 residuals may be page-locked host memory: refused before any launch if pageable
-  rc = device_readable(residuals_bf16, &rescore.rows.ptr, "ivf_pq");
-  if (rc != CRAG_OK) return rc;
-  return ivf_pq_passes(static_cast<const uint8_t*>(codes), code_stride, m, codebooks, lists, n_cand, k, rescore, out_ids,
-                       out_scores, out_minmax, plan, static_cast<cudaStream_t>(stream));
+  // Stage 1: the queries' tables, then the PQ scan for n_cand candidates, about two CTAs per SM in all; every
+  // (slice, query) CTA writes its part, so the merge reads `slices` parts.
+  const IvfPlan& ip = plan.cand.ivf;
+  const SearchPlan& sp = ip.scan;
+  const IvfArgs args{ip.work, ip.n_work, ip.list_mask, ip.coarse};
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return ivf_passes(nq, lists, n_cand, k, &rescore, out_ids, out_scores, out_minmax, ip, st, [&](int q0, int nqc, int& slices) {
+    const void* qp = rescore.queries.rows_from(q0, nqc).ptr;
+    pq_table_kernel<<<unsigned(nqc * m), kPqTableThreads, 0, st>>>(static_cast<const uint16_t*>(qp), dim, codebooks, m, plan.lut);
+    CRAG_CUDA_OK(cudaGetLastError());
+    slices = std::min(sp.grid, std::max(1, (2 * sp.grid + nqc - 1) / nqc));
+    int rc = CRAG_OK;
+    with_merge_tier(n_cand, [&](auto tier) {
+      constexpr int T = decltype(tier)::value;
+      rc = allow_dynamic_smem<pq_scan_kernel<T>>(PqScanSmem<T>::bytes(kPqMaxM));
+      if (rc != CRAG_OK) return;
+      pq_scan_kernel<T><<<unsigned(nqc * slices), kPqThreads, PqScanSmem<T>::bytes(m), st>>>(
+          static_cast<const uint8_t*>(codes), code_stride, m, plan.lut, slices, n_cand, args, sp.part_keys, sp.part_minmax);
+    });
+    if (rc != CRAG_OK) return rc;
+    CRAG_CUDA_OK(cudaGetLastError());
+    return CRAG_OK;
+  });
 }
 
 extern "C" int crag_pq_encode(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, const float* codebooks,
@@ -837,8 +826,7 @@ extern "C" int crag_pq_encode(const void* rows_bf16, int64_t n_rows, int dim, in
   rc = device_readable(rows_bf16, &rows, "pq_encode");
   if (rc != CRAG_OK) return rc;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  static bool attr_set[64] = {};
-  rc = allow_smem(pq_encode_kernel, pq_encode_smem_bytes(kPqMaxDsub), attr_set);
+  rc = allow_dynamic_smem<pq_encode_kernel>(pq_encode_smem_bytes(kPqMaxDsub));
   if (rc != CRAG_OK) return rc;
   constexpr int64_t kChunk = int64_t(1) << 22;   // rows per launch: (chunk / 128) * m blocks stay far below 2^31
   for (int64_t r0 = 0; r0 < n_rows; r0 += kChunk) {
@@ -916,25 +904,18 @@ extern "C" int crag_search_topk_b1(const void* bits, const float* alpha, int64_t
                                    int64_t row_offset, const void* queries_i8, const float* query_scales, int nq, int k,
                                    int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
                                    size_t workspace_bytes, crag_stream_t stream) {
-  if (nq < 1 || k < 1 || k > 128) return fail(CRAG_ERR_INVALID, "search_b1: need nq >= 1 and 1 <= k <= 128 (nq=%d k=%d)", nq, k);
-  if (dim8 < 128 || dim8 > 1024 || dim8 % 128 != 0) return fail(CRAG_ERR_INVALID, "search_b1: dim8 must be a multiple of 128 in [128, 1024] (dim8=%d)", dim8);
-  if (n_rows < 0 || n_rows >= (int64_t(1) << 31) - kTileRows) return fail(CRAG_ERR_INVALID, "search_b1: n_rows out of range (%lld)", (long long)n_rows);
-  if (row_stride < dim8 / 8 || row_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "search_b1: row_stride must be >= dim8 / 8 bytes and a multiple of 16 (row_stride=%lld)", (long long)row_stride);
-  if (n_rows > 0 && (!bits || !alpha)) return fail(CRAG_ERR_INVALID, "search_b1: null bits or alpha pointer");
-  if (reinterpret_cast<uintptr_t>(bits) & 15) return fail(CRAG_ERR_INVALID, "search_b1: bits must be 16-byte aligned");
-  if (!query_scales || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "search_b1: null query_scales or output pointer");
-  const Operand c{bits, n_rows, dim8 / 8, row_stride, kS8, "bits"}, q{queries_i8, nq, dim8, dim8, kS8, "queries_i8"};
-  const SearchPlan plan = plan_search(k, workspace);
-  int rc = check_operand("search_b1", q);
-  if (rc == CRAG_OK) rc = check_workspace("search_b1", workspace, workspace_bytes, plan.parts_bytes);
+  const Operand c{bits, n_rows, dim8 / 8, row_stride, kS8, "bits", true}, q{queries_i8, nq, dim8, dim8, kS8, "queries_i8"};
+  const SearchPlan plan = plan_search(k >= 1 && k <= 128 ? k : 1, workspace);
+  int rc = check_scan_args("search_b1", nq, k, 128, c, q, workspace, workspace_bytes, plan.parts_bytes);
   if (rc != CRAG_OK) return rc;
+  if ((n_rows > 0 && !alpha) || !query_scales || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "search_b1: null alpha, query_scales or output pointer");
   return topk_passes(c, q, k, row_offset, nullptr, B1Args{{alpha, query_scales}}, out_ids, out_scores, out_minmax,
                      nullptr, workspace_bytes, plan, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------ exact top-k for large k / many queries
-// Per chunk of queries: the wgmma GEMM writes the fp32 score block [q_chunk, ld] into the workspace
-// (gemm_scores_f32), then knn_select_kernel (knn_select.cuh) radix-selects each query's k best rows from its row.
+// Per chunk of queries the score block (score_block_chunks), then knn_select_kernel (knn_select.cuh) radix-selects each
+// query's k best rows from its row.
 namespace crag {
 namespace {
 inline int64_t knn_ld(int64_t n_rows) { return ((n_rows > 0 ? n_rows : 1) + 3) & ~int64_t(3); }
@@ -947,6 +928,29 @@ KnnWorkspace knn_workspace(int64_t n_rows, int q_chunk, void* ws = nullptr) {
   w.block = c.take<float>(size_t(q_chunk) * size_t(knn_ld(n_rows)));
   w.total = c.bytes;
   return w;
+}
+
+// Per chunk of queries, as many as the workspace holds score rows for: the wgmma GEMM writes the chunk's fp32 score
+// block [nqc, ld] into the workspace (gemm_scores_f32), then `select(q0, nqc, block, ld)` launches its per-query select.
+template <class Select>
+int score_block_chunks(const char* who, const Operand& corpus, const void* queries, int nq, void* workspace,
+                       size_t workspace_bytes, cudaStream_t stream, Select select) {
+  const int64_t ld = knn_ld(corpus.rows);
+  const size_t per_query = size_t(ld) * 4;
+  const size_t fit = workspace_bytes / per_query;
+  if (fit < 1) return fail(CRAG_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes (one query's score row)", who, workspace_bytes, per_query);
+  const int q_chunk = fit < size_t(nq) ? int(fit) : nq;
+  float* block = knn_workspace(corpus.rows, q_chunk, workspace).block;
+  const int dim = corpus.width;
+  for (int q0 = 0; q0 < nq; q0 += q_chunk) {
+    const int nqc = (nq - q0) < q_chunk ? (nq - q0) : q_chunk;
+    const int rc = gemm_scores_f32(static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, dim, corpus.ptr, corpus.stride,
+                                   block, ld, nqc, int(corpus.rows), dim, stream);
+    if (rc != CRAG_OK) return rc;
+    select(q0, nqc, block, ld);
+    CRAG_CUDA_OK(cudaGetLastError());
+  }
+  return CRAG_OK;
 }
 }  // namespace
 }  // namespace crag
@@ -964,23 +968,12 @@ extern "C" int crag_knn_topk(const void* corpus, int64_t n_rows, int dim, int64_
   int rc = check_scan_args("search", nq, k, kKnnMaxK, c, q, workspace, workspace_bytes, 0);
   if (rc != CRAG_OK) return rc;
   if (!out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "knn: null output pointer");
-  const int64_t ld = knn_ld(n_rows);
-  const size_t per_query = size_t(ld) * 4;
-  const size_t fit = workspace_bytes / per_query;
-  if (fit < 1) return fail(CRAG_ERR_WORKSPACE, "knn: workspace %zu < %zu bytes (one query's score row)", workspace_bytes, per_query);
-  const int q_chunk = fit < size_t(nq) ? int(fit) : nq;
-  float* block = knn_workspace(n_rows, q_chunk, workspace).block;
-  for (int q0 = 0; q0 < nq; q0 += q_chunk) {
-    const int nqc = (nq - q0) < q_chunk ? (nq - q0) : q_chunk;
-    rc = gemm_scores_f32(static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, dim, corpus, corpus_row_stride,
-                         block, ld, nqc, int(n_rows), dim, stream);
-    if (rc != CRAG_OK) return rc;
+  return score_block_chunks("knn", c, queries, nq, workspace, workspace_bytes, stream,
+                            [&](int q0, int nqc, const float* block, int64_t ld) {
     knn_select_kernel<<<nqc, kKnnThreads, 0, stream>>>(block, ld, int(n_rows), k, row_offset, out_ids + size_t(q0) * k,
                                                        out_scores + size_t(q0) * k,
                                                        out_minmax ? out_minmax + size_t(q0) * 2 : nullptr);
-    CRAG_CUDA_OK(cudaGetLastError());
-  }
-  return CRAG_OK;
+  });
 }
 
 // Threshold join: per chunk of queries the same score block as crag_knn_topk, then knn_threshold_kernel
@@ -1000,24 +993,13 @@ extern "C" int crag_knn_threshold(const void* corpus, int64_t n_rows, int dim, i
     return fail(CRAG_ERR_INVALID, "knn_threshold: need cap >= 1, 0 <= n_exclude <= %d and cap + n_exclude + 1 <= %d (cap=%d n_exclude=%d)",
                 kKnnMaxExclude, kKnnMaxK, cap, n_exclude);
   if (!out_counts || !out_ids || !out_scores || (n_exclude > 0 && !exclude_rows)) return fail(CRAG_ERR_INVALID, "knn_threshold: null pointer");
-  const int64_t ld = knn_ld(n_rows);
-  const size_t per_query = size_t(ld) * 4;
-  const size_t fit = workspace_bytes / per_query;
-  if (fit < 1) return fail(CRAG_ERR_WORKSPACE, "knn_threshold: workspace %zu < %zu bytes (one query's score row)", workspace_bytes, per_query);
-  const int q_chunk = fit < size_t(nq) ? int(fit) : nq;
-  float* block = knn_workspace(n_rows, q_chunk, workspace).block;
-  for (int q0 = 0; q0 < nq; q0 += q_chunk) {
-    const int nqc = (nq - q0) < q_chunk ? (nq - q0) : q_chunk;
-    rc = gemm_scores_f32(static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, dim, corpus, corpus_row_stride,
-                         block, ld, nqc, int(n_rows), dim, stream);
-    if (rc != CRAG_OK) return rc;
+  return score_block_chunks("knn_threshold", c, queries, nq, workspace, workspace_bytes, stream,
+                            [&](int q0, int nqc, const float* block, int64_t ld) {
     knn_threshold_kernel<<<nqc, kKnnThreads, 0, stream>>>(block, ld, int(n_rows), threshold, limit, cap,
                                                           self_rows ? self_rows + q0 : nullptr, exclude_rows, n_exclude,
                                                           out_counts + q0, out_ids + size_t(q0) * cap,
                                                           out_scores + size_t(q0) * cap);
-    CRAG_CUDA_OK(cudaGetLastError());
-  }
-  return CRAG_OK;
+  });
 }
 
 namespace crag {

@@ -27,6 +27,7 @@ import torch
 
 from . import _native
 from .index import DenseIndex, MAX_K
+from .quantized import _dim8, check_place, place_rows, quantize_rows, rescored_candidates
 
 TILE_ROWS = 128
 
@@ -214,53 +215,61 @@ class IVFIndex(_IVFSearch):
                             self._lib.crag_ivf_workspace_bytes(self.nlist, self.total_tiles, k), fine)
 
 
-class QuantizedIVF(_IVFSearch):
-    """Frozen int8 snapshot of an IVFIndex (crag_ivf_search_i8; DESIGN.md section 7).  Every stored residual row is
-    quantised to int8 with one fp32 scale; a search scans the probed tiles' int8 residuals for `candidates` positions
-    per query (S1 = int8 dot * scales + coarse term) and rescores those exactly from their bf16 residuals
-    (S2 = pinned-order fp32 dot + coarse term).  The fine pass reads dim8 + 4 bytes per probed stored row instead of
-    2 dim.  The bf16 residuals are read for the candidates only, so they may live in page-locked host memory."""
+class _RescoredIVF(_IVFSearch):
+    """A frozen snapshot of an IVFIndex whose fine pass scans a compressed copy of the stored residuals and rescores its
+    candidates exactly from the bf16 residuals (QuantizedIVF, pq.PQIVF).  Shares the IVFIndex's centroid table, list
+    layout and row ids; the bf16 residuals are read for the candidates only, so they may live in page-locked host
+    memory."""
 
-    def __init__(self, ivf: IVFIndex, residuals_bf16: torch.Tensor, residuals_i8: torch.Tensor, scales: torch.Tensor):
+    def __init__(self, ivf: IVFIndex, residuals_bf16: torch.Tensor):
         self.device, self.dim, self.nlist, self.n_rows = ivf.device, ivf.dim, ivf.nlist, ivf.n_rows
         self.centroids = ivf.centroids
         self.row_ids, self.list_tile_start, self.list_rows = ivf.row_ids, ivf.list_tile_start, ivf.list_rows
         self.total_tiles = ivf.total_tiles
         self._rows = residuals_bf16     # bf16 [total_tiles * 128, dim], on the device or in page-locked host memory
-        self._i8 = residuals_i8         # int8 [total_tiles * 128, dim8], device
-        self._scales = scales           # fp32 [total_tiles * 128], device; 0 on padding rows
-        self.dim8 = residuals_i8.shape[1]
         self._lib = _native.load()
-
-    @classmethod
-    def from_ivf(cls, ivf: IVFIndex, residuals: str = "device") -> "QuantizedIVF":
-        """Quantise `ivf`'s stored residuals.  residuals="device" shares the IVFIndex's bf16 residual buffer;
-        residuals="host" copies it into page-locked host memory."""
-        from .quantized import _dim8, quantize_rows
-        if residuals not in ("device", "host"):
-            raise ValueError('residuals must be "device" or "host"')
-        bf16 = ivf.residuals
-        i8, scales = quantize_rows(bf16, _dim8(ivf.dim))
-        if residuals == "host":
-            host = torch.empty(tuple(bf16.shape), dtype=torch.bfloat16, pin_memory=True)
-            host.copy_(bf16)
-            bf16 = host
-        with torch.cuda.device(ivf.device):
-            torch.cuda.current_stream(ivf.device).synchronize()   # the snapshot is complete when from_ivf returns
-        return cls(ivf, bf16, i8, scales)
 
     @property
     def residuals_on_device(self) -> bool:
         return self._rows.is_cuda
 
+    def _code_bytes(self) -> int:
+        """Device bytes of what the fine pass scans."""
+        raise NotImplementedError
+
     @property
     def device_bytes(self) -> int:
-        """Bytes of the fine index in device memory: int8 residuals, their scales and, with residuals="device", the
-        bf16 residuals (shared with the IVFIndex).  The centroid table, row_ids and list tables are not counted."""
-        b = self._i8.numel() + 4 * self._scales.numel()
+        """Bytes of the fine index in device memory: what the fine pass scans and, with residuals="device", the bf16
+        residuals (shared with the IVFIndex).  The centroid table, row_ids and list tables are not counted."""
+        b = self._code_bytes()
         if self._rows.is_cuda:
             b += 2 * self._rows.shape[0] * self._rows.stride(0) if self._rows.shape[0] else 0
         return b
+
+
+class QuantizedIVF(_RescoredIVF):
+    """Frozen int8 snapshot of an IVFIndex (crag_ivf_search_i8; DESIGN.md section 7).  Every stored residual row is
+    quantised to int8 with one fp32 scale; a search scans the probed tiles' int8 residuals for `candidates` positions
+    per query (S1 = int8 dot * scales + coarse term) and rescores those exactly from their bf16 residuals
+    (S2 = pinned-order fp32 dot + coarse term).  The fine pass reads dim8 + 4 bytes per probed stored row instead of
+    2 dim."""
+
+    def __init__(self, ivf: IVFIndex, residuals_bf16: torch.Tensor, residuals_i8: torch.Tensor, scales: torch.Tensor):
+        super().__init__(ivf, residuals_bf16)
+        self._i8 = residuals_i8         # int8 [total_tiles * 128, dim8], device
+        self._scales = scales           # fp32 [total_tiles * 128], device; 0 on padding rows
+        self.dim8 = residuals_i8.shape[1]
+
+    @classmethod
+    def from_ivf(cls, ivf: IVFIndex, residuals: str = "device") -> "QuantizedIVF":
+        """Quantise `ivf`'s stored residuals.  residuals="device" shares the IVFIndex's bf16 residual buffer;
+        residuals="host" copies it into page-locked host memory."""
+        check_place(residuals, "residuals")
+        i8, scales = quantize_rows(ivf.residuals, _dim8(ivf.dim))
+        return cls(ivf, place_rows(ivf.residuals, residuals, ivf.device), i8, scales)
+
+    def _code_bytes(self) -> int:
+        return self._i8.numel() + 4 * self._scales.numel()
 
     def search_device(self, queries_bf16: torch.Tensor, nprobe: int, k: int, candidates: Optional[int] = None,
                       stream: Optional[torch.cuda.Stream] = None, probed: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
@@ -268,11 +277,7 @@ class QuantizedIVF(_IVFSearch):
         (probed list ids int64 [nq, nprobe], their coarse scores fp32)), as IVFIndex.search_device.  Scores are the
         exact S2 values; minmax is (min, max) of the int8 stage's S1 over the probed rows.  candidates (default
         min(128, 4 k)) positions per query come from the int8 scan; 1 <= k <= candidates <= 128."""
-        if candidates is None:
-            candidates = min(MAX_K, 4 * k)
-        if not 1 <= k <= candidates <= MAX_K:
-            raise ValueError(f"need 1 <= k <= candidates <= {MAX_K} (k={k}, candidates={candidates})")
-        from .quantized import quantize_rows
+        candidates = rescored_candidates(k, candidates)
 
         def fine(q, p_ids, p_scores, ids, scores, minmax, ws, st):
             q8, qs = quantize_rows(q, self.dim8, st)

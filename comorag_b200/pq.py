@@ -17,8 +17,8 @@ from typing import Optional, Tuple
 import torch
 
 from . import _native
-from .index import MAX_K
-from .ivf import IVFIndex, _IVFSearch
+from .ivf import IVFIndex, _RescoredIVF
+from .quantized import check_place, place_rows, rescored_candidates
 
 CODEWORDS = 256
 MAX_M = 192          # one query's table, m * 256 * 4 bytes, fits in shared memory
@@ -83,21 +83,16 @@ def train_codebooks(sample_bf16: torch.Tensor, m: int, iters: int = 10, seed: in
     return cb
 
 
-class PQIVF(_IVFSearch):
+class PQIVF(_RescoredIVF):
     """Frozen product-quantized snapshot of an IVFIndex (crag_ivf_search_pq; DESIGN.md section 7).  Shares the
     IVFIndex's centroid table, list layout and row ids; holds the codes [n_rows_padded, code_stride(m)] and the
     codebooks [m, 256, dsub] on the device, and the bf16 residuals on the device or in page-locked host memory."""
 
     def __init__(self, ivf: IVFIndex, residuals_bf16: torch.Tensor, codes: torch.Tensor, codebooks: torch.Tensor):
-        self.device, self.dim, self.nlist, self.n_rows = ivf.device, ivf.dim, ivf.nlist, ivf.n_rows
-        self.centroids = ivf.centroids
-        self.row_ids, self.list_tile_start, self.list_rows = ivf.row_ids, ivf.list_tile_start, ivf.list_rows
-        self.total_tiles = ivf.total_tiles
+        super().__init__(ivf, residuals_bf16)
         self.m = codebooks.shape[0]
         self.codebooks = codebooks      # fp32 [m, 256, dsub], device
         self.codes = codes              # uint8 [total_tiles * 128, code_stride(m)], device; 0 on padding rows
-        self._rows = residuals_bf16     # bf16 [total_tiles * 128, dim], on the device or in page-locked host memory
-        self._lib = _native.load()
 
     @classmethod
     def from_ivf(cls, ivf: IVFIndex, m: int, codebooks: Optional[torch.Tensor] = None, train_rows: int = 1 << 20,
@@ -106,8 +101,7 @@ class PQIVF(_IVFSearch):
         stored rows drawn with `seed`; every rank of a row-sharded index passes the same codebooks.
         residuals="device" shares the IVFIndex's bf16 residual buffer; residuals="host" copies it into page-locked
         host memory."""
-        if residuals not in ("device", "host"):
-            raise ValueError('residuals must be "device" or "host"')
+        check_place(residuals, "residuals")
         check_shape(ivf.dim, m)
         bf16, dev = ivf.residuals, ivf.device
         real = torch.nonzero(ivf.row_ids >= 0).flatten()
@@ -120,26 +114,10 @@ class PQIVF(_IVFSearch):
             raise ValueError(f"codebooks must be [m, {CODEWORDS}, dim / m] = [{m}, {CODEWORDS}, {ivf.dim // m}]")
         codes = encode(bf16, codebooks)
         codes[ivf.row_ids < 0] = 0                                      # padding rows: code 0, never scored
-        if residuals == "host":
-            host = torch.empty(tuple(bf16.shape), dtype=torch.bfloat16, pin_memory=True)
-            host.copy_(bf16)
-            bf16 = host
-        with torch.cuda.device(dev):
-            torch.cuda.current_stream(dev).synchronize()   # the snapshot is complete when from_ivf returns
-        return cls(ivf, bf16, codes, codebooks)
+        return cls(ivf, place_rows(bf16, residuals, dev), codes, codebooks)
 
-    @property
-    def residuals_on_device(self) -> bool:
-        return self._rows.is_cuda
-
-    @property
-    def device_bytes(self) -> int:
-        """Bytes of the fine index in device memory: codes, codebooks and, with residuals="device", the bf16 residuals
-        (shared with the IVFIndex).  The centroid table, row_ids and list tables are not counted."""
-        b = self.codes.numel() + 4 * self.codebooks.numel()
-        if self._rows.is_cuda:
-            b += 2 * self._rows.shape[0] * self._rows.stride(0) if self._rows.shape[0] else 0
-        return b
+    def _code_bytes(self) -> int:
+        return self.codes.numel() + 4 * self.codebooks.numel()
 
     def search_device(self, queries_bf16: torch.Tensor, nprobe: int, k: int, candidates: Optional[int] = None,
                       stream: Optional[torch.cuda.Stream] = None, probed: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
@@ -147,10 +125,7 @@ class PQIVF(_IVFSearch):
         (probed list ids int64 [nq, nprobe], their coarse scores fp32)), as IVFIndex.search_device.  Scores are the
         exact S2 values; minmax is (min, max) of the PQ stage's S1 over the probed rows.  candidates (default
         min(128, 4 k)) positions per query come from the PQ scan; 1 <= k <= candidates <= 128."""
-        if candidates is None:
-            candidates = min(MAX_K, 4 * k)
-        if not 1 <= k <= candidates <= MAX_K:
-            raise ValueError(f"need 1 <= k <= candidates <= {MAX_K} (k={k}, candidates={candidates})")
+        candidates = rescored_candidates(k, candidates)
 
         def fine(q, p_ids, p_scores, ids, scores, minmax, ws, st):
             _native.check(self._lib.crag_ivf_search_pq(

@@ -8,7 +8,7 @@ Semantics: DESIGN.md section 3e and oracle/quant_oracle.py.
 """
 from __future__ import annotations
 
-from typing import Optional, Tuple
+from typing import Callable, Optional, Tuple
 
 import numpy as np
 import torch
@@ -21,24 +21,59 @@ def _dim8(dim: int) -> int:
     return (dim + 127) // 128 * 128
 
 
-def quantize_rows(rows: torch.Tensor, dim8: int, stream: Optional[torch.cuda.Stream] = None
-                  ) -> Tuple[torch.Tensor, torch.Tensor]:
-    """crag_quantize_rows_i8 of a device bf16 [n, dim] tensor (unit inner stride): (int8 [n, dim8], fp32 scales [n])."""
+def _encode_rows(name: str, fn: str, rows: torch.Tensor, width: Callable[[int], int], dtype: torch.dtype,
+                 stream: Optional[torch.cuda.Stream]) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The C row encoder `fn` behind the public `name` of a device bf16 [n, dim] tensor (unit inner stride): (codes
+    `dtype` [n, width(dim)], fp32 per-row scales [n])."""
     if rows.dtype != torch.bfloat16 or rows.dim() != 2 or not rows.is_cuda or (rows.shape[0] > 1 and rows.stride(1) != 1):
-        raise ValueError("quantize_rows expects a CUDA bf16 [n, dim] tensor with unit inner stride")
+        raise ValueError(f"{name} expects a CUDA bf16 [n, dim] tensor with unit inner stride")
     n, dim = rows.shape
+    width = width(dim)
     dev = rows.device
-    lib = _native.load()
     with torch.cuda.device(dev):
         st = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.stream(st):
-            out = torch.empty((n, dim8), dtype=torch.int8, device=dev)
+            codes = torch.empty((n, width), dtype=dtype, device=dev)
             scales = torch.empty((n,), dtype=torch.float32, device=dev)
-            rc = lib.crag_quantize_rows_i8(rows.data_ptr() if n else 0, n, dim, rows.stride(0) if n else dim,
-                                           out.data_ptr() if n else 0, dim8, scales.data_ptr() if n else 0,
-                                           st.cuda_stream)
-            _native.check(rc, "crag_quantize_rows_i8")
-    return out, scales
+            rc = getattr(_native.load(), fn)(rows.data_ptr() if n else 0, n, dim, rows.stride(0) if n else dim,
+                                             codes.data_ptr() if n else 0, width, scales.data_ptr() if n else 0,
+                                             st.cuda_stream)
+            _native.check(rc, fn)
+    return codes, scales
+
+
+def quantize_rows(rows: torch.Tensor, dim8: int, stream: Optional[torch.cuda.Stream] = None
+                  ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """crag_quantize_rows_i8 of a device bf16 [n, dim] tensor (unit inner stride): (int8 [n, dim8], fp32 scales [n])."""
+    return _encode_rows("quantize_rows", "crag_quantize_rows_i8", rows, lambda dim: dim8, torch.int8, stream)
+
+
+def check_place(where: str, arg: str) -> None:
+    """A snapshot's bf16 rows live on the "device" or in page-locked "host" memory; `arg` names the argument."""
+    if where not in ("device", "host"):
+        raise ValueError(f'{arg} must be "device" or "host"')
+
+
+def place_rows(rows_bf16: torch.Tensor, where: str, device: torch.device) -> torch.Tensor:
+    """The bf16 rows a snapshot keeps: `rows_bf16` itself (where="device") or a copy in page-locked host memory
+    (where="host").  Synchronises `device`'s current stream, so the snapshot is complete when this returns."""
+    if where == "host":
+        host = torch.empty(tuple(rows_bf16.shape), dtype=torch.bfloat16, pin_memory=True)
+        if rows_bf16.numel():
+            host.copy_(rows_bf16)
+        rows_bf16 = host
+    with torch.cuda.device(device):
+        torch.cuda.current_stream(device).synchronize()
+    return rows_bf16
+
+
+def rescored_candidates(k: int, candidates: Optional[int]) -> int:
+    """Stage-1 candidates per query of a rescored search: default min(128, 4 k), and 1 <= k <= candidates <= 128."""
+    if candidates is None:
+        candidates = min(MAX_K, 4 * k)
+    if not 1 <= k <= candidates <= MAX_K:
+        raise ValueError(f"need 1 <= k <= candidates <= {MAX_K} (k={k}, candidates={candidates})")
+    return candidates
 
 
 class QuantizedIndex:
@@ -77,21 +112,13 @@ class QuantizedIndex:
     def from_dense(cls, index: DenseIndex, rows: str = "device") -> "QuantizedIndex":
         """Quantise the rows `index` holds now.  rows="device" keeps a reference to the index's bf16 buffer;
         rows="host" copies the bf16 rows into page-locked host memory, so the DenseIndex may be dropped."""
-        if rows not in ("device", "host"):
-            raise ValueError('rows must be "device" or "host"')
+        check_place(rows, "rows")
         buf, n = index._snapshot()
         dev = index.device
         bf16 = buf[:n]
         codes, scales = cls._encode(bf16 if n else torch.zeros((0, index.dim_pad), dtype=torch.bfloat16, device=dev),
                                     _dim8(index.dim_pad))
-        if rows == "host":
-            host = torch.empty((n, index.dim_pad), dtype=torch.bfloat16, pin_memory=True)
-            if n:
-                host.copy_(bf16)
-            bf16 = host
-        with torch.cuda.device(dev):
-            torch.cuda.current_stream(dev).synchronize()   # the snapshot is complete when from_dense returns
-        return cls(bf16, codes, scales, index.dim, dev, index.row_offset)
+        return cls(place_rows(bf16, rows, dev), codes, scales, index.dim, dev, index.row_offset)
 
     @property
     def n_rows(self) -> int:
@@ -118,10 +145,7 @@ class QuantizedIndex:
         """Top k of a device bf16 [nq, dim_pad] query block: (ids int64 [nq, k], scores fp32 [nq, k]) on the device.
         Scores are the exact fp32 dots of the rescore (descending, ties by ascending id); -1 / -inf where fewer than
         k rows exist.  candidates (default min(128, 4 k)) rows per query come from the scan of the code rows."""
-        if candidates is None:
-            candidates = min(MAX_K, 4 * k)
-        if not (1 <= k <= candidates <= MAX_K):
-            raise ValueError(f"need 1 <= k <= candidates <= {MAX_K} (k={k}, candidates={candidates})")
+        candidates = rescored_candidates(k, candidates)
         if queries.dtype != torch.bfloat16 or queries.dim() != 2 or queries.shape[1] != self.dim_pad or not queries.is_cuda:
             raise ValueError(f"queries must be device bf16 [nq, {self.dim_pad}]")
         queries = queries.contiguous()

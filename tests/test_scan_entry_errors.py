@@ -1,8 +1,9 @@
 """Argument validation of every C entry point of the shard scan, without a device: the flat bf16 and int8 top-k scans,
-the one-pass scan, the score-all pass, the IVF assignment, both IVF searches and the exact large-k top-k.  Each case
-breaks exactly one argument of an otherwise valid call and must be refused before any launch with INVALID (or
-WORKSPACE for a short workspace) and a crag_last_error() naming that argument.  The host buffer passed as every
-pointer is never dereferenced.  Pageable-memory refusals need a device and are tested in test_ivf_i8_gpu.py."""
+the one-bit scan, the one-pass scan, the score-all pass, the IVF assignment, the bf16, int8 and PQ IVF searches, the PQ
+encode, the exact large-k top-k and the threshold join.  Each case breaks exactly one argument of an otherwise valid
+call and must be refused before any launch with INVALID (or WORKSPACE for a short workspace) and a crag_last_error()
+naming that argument.  The host buffer passed as every pointer is never dereferenced.  Pageable-memory refusals need a
+device and are tested in test_ivf_i8_gpu.py and test_ivf_pq_gpu.py."""
 import ctypes as C
 
 import pytest
@@ -222,3 +223,104 @@ def test_ivf_search_i8(lib, p):
     expect(lib, call(ws_bytes=16), WORKSPACE, "workspace")
     short = lib.crag_ivf_i8_workspace_bytes(8, 8, 40) - 256
     expect(lib, call(ws_bytes=short), WORKSPACE, "workspace")
+
+
+def test_topk_b1(lib, p):
+    call = caller(lib, "crag_search_topk_b1", [
+        ("bits", p), ("alpha", p), ("n_rows", 1000), ("dim8", 1024), ("stride", 128), ("row_offset", 0),
+        ("queries", p), ("query_scales", p), ("nq", 4), ("k", 10), ("ids", p), ("scores", p), ("minmax", p),
+        ("ws", p), ("ws_bytes", 1 << 24), ("stream", None)])
+    expect(lib, call(nq=0), INVALID, "nq")
+    expect(lib, call(k=0), INVALID, "k=")
+    expect(lib, call(k=129), INVALID, "k=")
+    for dim8 in (0, 192, 1000, 2048):
+        expect(lib, call(dim8=dim8), INVALID, "dim8")
+    expect(lib, call(stride=120), INVALID, "row_stride")
+    expect(lib, call(stride=136), INVALID, "row_stride")
+    expect(lib, call(n_rows=-1), INVALID, "n_rows")
+    expect(lib, call(n_rows=1 << 31), INVALID, "n_rows")
+    expect(lib, call(bits=None), INVALID, "bits")
+    expect(lib, call(alpha=None), INVALID, "alpha")
+    for name in ("bits", "alpha", "queries", "query_scales", "ids", "scores", "ws"):
+        expect(lib, call(**{name: None}), INVALID, "null")
+    expect(lib, call(bits=p + 8), INVALID, "aligned")
+    expect(lib, call(queries=p + 8), INVALID, "aligned")
+    expect(lib, call(ws=p + 64), INVALID, "workspace")
+    expect(lib, call(ws_bytes=16), WORKSPACE, "workspace")
+
+
+def test_ivf_search_pq(lib, p):
+    call = caller(lib, "crag_ivf_search_pq", [
+        ("codes", p), ("m", 8), ("code_stride", 16), ("codebooks", p), ("res_bf16", p), ("dim", 768), ("stride", 768),
+        ("n_rows_padded", 1024), ("list_tile_start", p), ("list_rows", p), ("nlist", 8), ("total_tiles", 8),
+        ("row_ids", p), ("queries_bf16", p), ("nq", 4), ("probed_ids", p), ("probed_scores", p), ("nprobe", 2),
+        ("n_cand", 40), ("k", 10), ("ids", p), ("scores", p), ("minmax", p), ("ws", p), ("ws_bytes", 1 << 24),
+        ("stream", None)])
+    expect(lib, call(nq=0), INVALID, "nq")
+    expect(lib, call(k=0), INVALID, "n_cand")
+    expect(lib, call(k=41), INVALID, "n_cand")
+    expect(lib, call(n_cand=129), INVALID, "n_cand")
+    expect(lib, call(nprobe=0), INVALID, "nprobe")
+    expect(lib, call(nprobe=9), INVALID, "nprobe")
+    expect(lib, call(nlist=0), INVALID, "nlist")
+    expect(lib, call(total_tiles=7), INVALID, "total_tiles")
+    expect(lib, call(n_rows_padded=100), INVALID, "n_rows_padded")
+    expect(lib, call(total_tiles=0, n_rows_padded=0), INVALID, "empty")
+    for m in (0, 7, 193):
+        expect(lib, call(m=m), INVALID, "m must divide")
+    expect(lib, call(m=192), INVALID, "code_stride")
+    expect(lib, call(dim=100), INVALID, "dim")
+    expect(lib, call(dim=2048, stride=2048), INVALID, "dim")
+    expect(lib, call(code_stride=8), INVALID, "code_stride")
+    expect(lib, call(code_stride=24), INVALID, "code_stride")
+    expect(lib, call(codes=None), INVALID, "codes")
+    expect(lib, call(codebooks=None), INVALID, "codebooks")
+    for name in ("codes", "codebooks", "list_tile_start", "list_rows", "row_ids", "probed_ids", "probed_scores", "ids",
+                 "scores", "ws"):
+        expect(lib, call(**{name: None}), INVALID, "null")
+    for name in ("codes", "codebooks"):
+        expect(lib, call(**{name: p + 4}), INVALID, "aligned")
+    expect(lib, call(ws=p + 64), INVALID, "workspace")
+    expect(lib, call(ws_bytes=16), WORKSPACE, "workspace")
+    short = lib.crag_ivf_pq_workspace_bytes(8, 8, 40, 8) - 256
+    expect(lib, call(ws_bytes=short), WORKSPACE, "workspace")
+
+
+def test_pq_encode(lib, p):
+    call = caller(lib, "crag_pq_encode", [("rows", p), ("n_rows", 10), ("dim", 768), ("stride", 768),
+                                          ("codebooks", p), ("m", 8), ("codes", p), ("code_stride", 16),
+                                          ("stream", None)])
+    for m in (0, 5, 193):
+        expect(lib, call(m=m), INVALID, "m must divide")
+    expect(lib, call(dim=96), INVALID, "dim")
+    expect(lib, call(dim=2048, stride=2048), INVALID, "dim")
+    expect(lib, call(n_rows=-1), INVALID, "n_rows")
+    expect(lib, call(n_rows=1 << 31), INVALID, "n_rows")
+    expect(lib, call(stride=512), INVALID, "row_stride")
+    expect(lib, call(code_stride=4), INVALID, "code_stride")
+    for name in ("rows", "codebooks", "codes"):
+        expect(lib, call(**{name: None}), INVALID, name)
+    expect(lib, call(rows=p + 1), INVALID, "aligned")
+    expect(lib, call(codebooks=p + 2), INVALID, "aligned")
+
+
+def test_knn_threshold(lib, p):
+    call = caller(lib, "crag_knn_threshold", [
+        ("corpus", p), ("n_rows", 1000), ("dim", 1024), ("stride", 1024), ("queries", p), ("nq", 4),
+        ("threshold", 0.5), ("limit", 10), ("cap", 5), ("self_rows", None), ("exclude", p), ("n_exclude", 0),
+        ("counts", p), ("ids", p), ("scores", p), ("ws", p), ("ws_bytes", 1 << 24), ("stream", None)])
+    for case in BF16_CASES:
+        kw, code, word = rebase(p, case)
+        expect(lib, call(**kw), code, word)
+    for t in (float("nan"), float("inf"), float("-inf")):
+        expect(lib, call(threshold=t), INVALID, "threshold")
+    expect(lib, call(limit=0), INVALID, "k=")
+    expect(lib, call(cap=0), INVALID, "cap")
+    expect(lib, call(cap=2048), INVALID, "cap")
+    expect(lib, call(n_exclude=-1), INVALID, "n_exclude")
+    expect(lib, call(n_exclude=65), INVALID, "n_exclude")
+    expect(lib, call(cap=2048 - 64, n_exclude=64), INVALID, "cap")
+    expect(lib, call(n_exclude=3, exclude=None), INVALID, "null")
+    for name in ("counts", "ids", "scores"):
+        expect(lib, call(**{name: None}), INVALID, "null")
+    expect(lib, call(ws_bytes=1000 * 4 - 1), WORKSPACE, "workspace")
