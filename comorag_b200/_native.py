@@ -97,6 +97,13 @@ SIGNATURES = {
     "crag_search_topk_b1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_void_p,
                                       C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_size_t, C.c_void_p]),
+    "crag_knn_code_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "crag_knn_topk_i8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_void_p,
+                                   C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_size_t, C.c_void_p]),
+    "crag_knn_topk_b1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_void_p,
+                                   C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_size_t, C.c_void_p]),
     "crag_ivf_i8_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int]),
     "crag_ivf_search_i8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int64,
                                      C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,

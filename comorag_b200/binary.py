@@ -2,8 +2,9 @@
 
 Every row is stored as its sign bits plus one fp32 scale, alpha = mean |x_i|: 132 bytes per row at dim 1024, against
 2048 for bf16 and 1028 for int8.  A search quantises the queries to int8 (crag_quantize_rows_i8), runs
-crag_search_topk_b1 over the codes for `candidates` rows per query, then crag_rescore_topk recomputes each candidate's
-score from its bf16 row and the bf16 query and keeps the best k, as QuantizedIndex does.  The returned scores are those
+crag_search_topk_b1 (crag_knn_topk_b1 above 128 candidates, search_wide) over the codes for `candidates` rows per
+query, then crag_rescore_topk recomputes each candidate's score from its bf16 row and the bf16 query and keeps the best
+k, as QuantizedIndex does.  The returned scores are those
 exact fp32 dots; only the choice of candidates comes from the one-bit scores.  The bf16 rows may live in page-locked
 host memory (rows="host").  Semantics: DESIGN.md section 3f and tests/binary_oracle.py.
 """
@@ -13,7 +14,6 @@ from typing import Optional, Tuple
 
 import torch
 
-from . import _native
 from .quantized import QuantizedIndex, _dim8, _encode_rows
 
 
@@ -25,18 +25,13 @@ def binarize_rows(rows: torch.Tensor, stream: Optional[torch.cuda.Stream] = None
 
 class BinaryIndex(QuantizedIndex):
     """Frozen one-bit snapshot of a DenseIndex's rows (rows added to the DenseIndex later are not seen).  The surface
-    is QuantizedIndex's: from_dense(index, rows="device" | "host"), search_device, search, prepare_queries, n_rows,
-    rows_on_device and device_bytes."""
+    is QuantizedIndex's: from_dense(index, rows="device" | "host"), search_device, search, search_device_wide,
+    search_wide, prepare_queries, n_rows, rows_on_device and device_bytes."""
 
     @staticmethod
     def _encode(rows: torch.Tensor, dim8: int) -> Tuple[torch.Tensor, torch.Tensor]:
         return binarize_rows(rows)
 
-    def _scan(self, q8: torch.Tensor, qs: torch.Tensor, candidates: int, c_ids: torch.Tensor, c_sc: torch.Tensor,
-              ws: torch.Tensor, st: torch.cuda.Stream) -> None:
-        n, nq = self.n_rows, q8.shape[0]
-        rc = _native.load().crag_search_topk_b1(self._codes.data_ptr() if n else 0, self._scales.data_ptr() if n else 0,
-                                                n, self.dim8, self._codes.shape[1], self.row_offset, q8.data_ptr(),
-                                                qs.data_ptr(), nq, candidates, c_ids.data_ptr(), c_sc.data_ptr(), 0,
-                                                ws.data_ptr(), ws.numel(), st.cuda_stream)
-        _native.check(rc, "crag_search_topk_b1")
+    @staticmethod
+    def _stage1(wide: bool) -> str:
+        return "crag_knn_topk_b1" if wide else "crag_search_topk_b1"

@@ -9,21 +9,19 @@
 //   2. gather, one pass in row order: every row above T goes to the candidate list, and the FIRST `quota` rows equal
 //      to T in ascending row order (a running block-wide exclusive scan per tile of rows, which stops once the quota
 //      is met) -- ties then resolve to ascending row ids exactly, as make_key orders them;
-//   3. bitonic sort of the <= 2048 collected keys in shared memory (16 KB), ids row + row_offset out.
+//   3. bitonic sort of the <= 2048 collected keys in shared memory (16 KB, knn_sort.cuh), ids row + row_offset out.
 // (min, max) over all rows is reduced in the gather pass.  n_rows <= k skips step 1 and sorts every row.
 // Pure SIMT code with no wgmma / TMA / mbarrier in it, so tests/warp_emu runs this very header on emulated blocks.
 #pragma once
 #include <stdint.h>
 #include <cuda_runtime.h>
 
+#include "knn_sort.cuh"
 #include "topk.cuh"
 
 namespace crag {
 namespace {
 
-constexpr int kKnnMaxK = 2048;
-constexpr int kKnnThreads = 512;
-constexpr int kKnnWarps = kKnnThreads / 32;
 constexpr int kKnnBins = 2048;
 constexpr int kKnnLoads = 4;   // 16-byte loads per thread in flight in a histogram pass
 
@@ -48,30 +46,6 @@ __device__ __forceinline__ int knn_block_exclusive_scan(int v, int* s_warp, int*
   __syncthreads();   // s_warp is free for the next call
   *total = all;
   return before + x - v;
-}
-
-// ---- 3. bitonic sort (descending) of s_keys[0, count), zero-padded to a power of two; ends with the block synced
-__device__ __forceinline__ void knn_bitonic_sort(uint64_t* s_keys, int count, int tid) {
-  int n2 = 1;
-  while (n2 < count) n2 <<= 1;
-  __syncthreads();
-  for (int i = count + tid; i < n2; i += kKnnThreads) s_keys[i] = 0ull;
-  __syncthreads();
-  for (int size = 2; size <= n2; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int p = tid; p < (n2 >> 1); p += kKnnThreads) {
-        const int a = 2 * p - (p & (stride - 1));   // p with a zero bit inserted at `stride`
-        const int b = a + stride;
-        const uint64_t ka = s_keys[a], kb = s_keys[b];
-        const bool desc = (a & size) == 0;
-        if ((ka < kb) == desc) {
-          s_keys[a] = kb;
-          s_keys[b] = ka;
-        }
-      }
-      __syncthreads();
-    }
-  }
 }
 
 // scores: fp32 rows of `ld` floats (ld % 4 == 0, 16-byte aligned), block q reads row q; outputs [gridDim.x, k].

@@ -79,7 +79,7 @@ extern "C" int crag_binarize_rows(const void* rows_bf16, int64_t n_rows, int dim
 extern "C" int crag_rescore_topk(const void* rows_bf16, int64_t n_rows, int dim, int64_t row_stride, int64_t row_offset,
                                  const void* queries_bf16, int nq, const int64_t* cand_ids, int n_cand, int k,
                                  int64_t* out_ids, float* out_scores, crag_stream_t stream) {
-  if (nq < 1 || n_cand < 1 || n_cand > kRescoreMaxCand || k < 1 || k > n_cand) return fail(CRAG_ERR_INVALID, "rescore: need nq >= 1 and 1 <= k <= n_cand <= %d (nq=%d n_cand=%d k=%d)", kRescoreMaxCand, nq, n_cand, k);
+  if (nq < 1 || n_cand < 1 || n_cand > kKnnMaxK || k < 1 || k > n_cand) return fail(CRAG_ERR_INVALID, "rescore: need nq >= 1 and 1 <= k <= n_cand <= %d (nq=%d n_cand=%d k=%d)", kKnnMaxK, nq, n_cand, k);
   if (dim < 8 || dim > 1024 || dim % 8 != 0) return fail(CRAG_ERR_INVALID, "rescore: dim must be a multiple of 8 in [8, 1024] (dim=%d)", dim);
   if (n_rows < 0 || n_rows >= (int64_t(1) << 31) || row_offset < 0) return fail(CRAG_ERR_INVALID, "rescore: need 0 <= n_rows < 2^31 and row_offset >= 0");
   if (row_stride < dim || row_stride % 8 != 0) return fail(CRAG_ERR_INVALID, "rescore: row_stride must be >= dim and a multiple of 8");
@@ -90,9 +90,13 @@ extern "C" int crag_rescore_topk(const void* rows_bf16, int64_t n_rows, int dim,
     const int rc = device_readable(rows_bf16, &rows, "rescore");
     if (rc != CRAG_OK) return rc;
   }
-  rescore_topk_kernel<<<nq, kRescoreThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint16_t*>(rows), n_rows, dim, row_stride, row_offset, static_cast<const uint16_t*>(queries_bf16),
-      cand_ids, n_cand, k, out_ids, out_scores);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const uint16_t* r = static_cast<const uint16_t*>(rows);
+  const uint16_t* qb = static_cast<const uint16_t*>(queries_bf16);
+  if (n_cand <= kRescoreMaxCand)   // one warp sorts the keys in registers
+    rescore_topk_kernel<<<nq, kRescoreThreads, 0, st>>>(r, n_rows, dim, row_stride, row_offset, qb, cand_ids, n_cand, k, out_ids, out_scores);
+  else                             // a block sorts them in shared memory
+    rescore_wide_kernel<<<nq, kKnnThreads, 0, st>>>(r, n_rows, dim, row_stride, row_offset, qb, cand_ids, n_cand, k, out_ids, out_scores);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }

@@ -8,7 +8,8 @@
 //             order: lane l of a warp takes the 16-byte chunks l, l + 32, ...; inside a chunk each product (rounded)
 //             is added to the lane's partial (rounded) in element order from 0.f; the partials are combined by an
 //             xor-shuffle tree over 16, 8, 4, 2, 1.  The result is the top k of the candidates by (score descending,
-//             row ascending), as make_key orders them.
+//             row ascending), as make_key orders them: up to 128 candidates one warp sorts the keys in registers, up to
+//             2048 a block sorts them in shared memory (knn_sort.cuh).
 //   binarize  (one-bit shards, crag_search_topk_b1, DESIGN.md 3f) a bf16 row x of width dim becomes dim8 / 8 code bytes,
 //             bit j of byte b set iff x_(8 b + j) > 0 (zeros, -0 and the padding columns dim .. dim8 - 1 give 0, read as
 //             -1), and alpha = sum |x_i| / dim (division rounded to nearest), the sum taken in the rescore's order
@@ -23,6 +24,7 @@
 
 #include <type_traits>
 
+#include "knn_sort.cuh"
 #include "pool_floor.cuh"   // kNQ, kTileRows
 #include "topk.cuh"
 
@@ -132,6 +134,32 @@ __device__ __forceinline__ int list_of_position(const int32_t* __restrict__ list
   return lo;
 }
 
+// The rescore key of one candidate, by one warp (all lanes return it): make_key(S2, local) for the candidate at local
+// row `local` of rows (bf16 [n_rows, row_stride], device or page-locked host memory) against the query qv (bf16 [dim],
+// n_chunks = dim / 8, 16-byte aligned), S2 summed in the pinned order; 0 (no candidate) for a local row outside
+// [0, n_rows), whose row is never read.  q: the query's index in the coarse table of an IVF pass.
+template <class ListTerm>
+__device__ __forceinline__ uint64_t rescore_key(const uint16_t* __restrict__ rows, int64_t n_rows, int n_chunks,
+                                                int64_t row_stride, const uint16_t* __restrict__ qv, int64_t local,
+                                                int q, int lane, const ListTerm& lists) {
+  uint64_t key = 0;   // no candidate
+  if (local >= 0 && local < n_rows) {   // warp-uniform
+    const uint16_t* xr = rows + local * row_stride;
+    float partial = 0.f;
+#pragma unroll 4
+    for (int ch = lane; ch < n_chunks; ch += 32)
+      partial = dot_chunk(partial, *reinterpret_cast<const uint4*>(xr + ch * 8), __ldg(reinterpret_cast<const uint4*>(qv + ch * 8)));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) partial = __fadd_rn(partial, __shfl_xor_sync(0xffffffffu, partial, o));
+    if constexpr (std::is_same<ListTerm, IvfListTerm>::value) {
+      const int l = list_of_position(lists.list_tile_start, lists.nlist, local);
+      partial = __fadd_rn(partial, __ldg(&lists.coarse[int64_t(l) * kNQ + q]));
+    }
+    key = make_key(partial, uint32_t(local));
+  }
+  return key;
+}
+
 // The body of both rescore kernels; one CTA per query.  rows: bf16 [n_rows, row_stride] (device or page-locked host
 // memory), queries: bf16 [nq, dim] dense, dim a multiple of 8, rows and queries 16-byte aligned.  cand_ids: int64
 // [nq, n_cand] global ids; an id outside [row_offset, row_offset + n_rows) -- -1 among them -- is no candidate and its
@@ -149,22 +177,8 @@ __device__ __forceinline__ void rescore_topk_body(const uint16_t* __restrict__ r
   const uint16_t* qv = queries + int64_t(q) * dim;
   const int n_chunks = dim / 8;
   for (int c = warp; c < kRescoreMaxCand; c += kRescoreThreads / 32) {
-    uint64_t key = 0;   // no candidate
     const int64_t local = c < n_cand ? __ldg(&cand_ids[int64_t(q) * n_cand + c]) - row_offset : -1;
-    if (local >= 0 && local < n_rows) {   // warp-uniform
-      const uint16_t* xr = rows + local * row_stride;
-      float partial = 0.f;
-#pragma unroll 4
-      for (int ch = lane; ch < n_chunks; ch += 32)
-        partial = dot_chunk(partial, *reinterpret_cast<const uint4*>(xr + ch * 8), __ldg(reinterpret_cast<const uint4*>(qv + ch * 8)));
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) partial = __fadd_rn(partial, __shfl_xor_sync(0xffffffffu, partial, o));
-      if constexpr (std::is_same<ListTerm, IvfListTerm>::value) {
-        const int l = list_of_position(lists.list_tile_start, lists.nlist, local);
-        partial = __fadd_rn(partial, __ldg(&lists.coarse[int64_t(l) * kNQ + q]));
-      }
-      key = make_key(partial, uint32_t(local));
-    }
+    const uint64_t key = rescore_key(rows, n_rows, n_chunks, row_stride, qv, local, q, lane, lists);
     if (lane == 0) keys[c] = key;
   }
   __syncthreads();
@@ -199,6 +213,29 @@ ivf_rescore_topk_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int d
                         const uint16_t* __restrict__ queries, const int64_t* __restrict__ cand_ids, int n_cand, int k,
                         int64_t* __restrict__ out_ids, float* __restrict__ out_scores, const IvfListTerm lists) {
   rescore_topk_body(rows, n_rows, dim, row_stride, int64_t(0), queries, cand_ids, n_cand, k, out_ids, out_scores, lists);
+}
+
+// crag_rescore_topk above 128 candidates (n_cand <= kKnnMaxK): one CTA of kKnnThreads per query, one warp per candidate
+// (rescore_key, as rescore_topk_kernel computes it), the keys in shared memory (16 KB at 2048) sorted by
+// knn_bitonic_sort, the top k out; -1 / -inf past the valid candidates.
+__global__ void __launch_bounds__(kKnnThreads)
+rescore_wide_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride, int64_t row_offset,
+                    const uint16_t* __restrict__ queries, const int64_t* __restrict__ cand_ids, int n_cand, int k,
+                    int64_t* __restrict__ out_ids, float* __restrict__ out_scores) {
+  __shared__ uint64_t s_keys[kKnnMaxK];
+  const int q = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint16_t* qv = queries + int64_t(q) * dim;
+  const int64_t* cand = cand_ids + int64_t(q) * n_cand;
+  for (int c = warp; c < n_cand; c += kKnnWarps) {
+    const uint64_t key = rescore_key(rows, n_rows, dim / 8, row_stride, qv, __ldg(&cand[c]) - row_offset, q, lane, NoListTerm{});
+    if (lane == 0) s_keys[c] = key;
+  }
+  knn_bitonic_sort(s_keys, n_cand, tid);
+  for (int j = tid; j < k; j += kKnnThreads) {
+    const uint64_t key = s_keys[j];
+    out_ids[int64_t(q) * k + j] = key ? int64_t(key_id(key)) + row_offset : -1;
+    out_scores[int64_t(q) * k + j] = key ? key_score(key) : -INFINITY;
+  }
 }
 
 }  // namespace crag

@@ -27,7 +27,7 @@
 // Variants of the same pipeline, named by the kernel's argument struct: IvfArgs walks a work-list of probed tiles
 // (crag_ivf_search); ScoreArgs stores every score (crag_search_scores) or keeps each row's running argmax over centroid
 // blocks (crag_ivf_assign); I8Args scans int8 rows (crag_search_topk_i8), I8IvfArgs int8 IVF lists (crag_ivf_search_i8),
-// B1Args one-bit rows (crag_search_topk_b1).
+// B1Args one-bit rows (crag_search_topk_b1), CodeScoreArgs every S1 of int8 or one-bit rows (crag_knn_topk_i8 / _b1).
 // Around it in this file: the per-shard merge (merge_topk_kernel), the fused
 // finalize + NVLink exchange + global merge of the row-sharded index
 // (finalize_exchange_kernel), the C-ABI entry points, and crag_knn_topk -- exact
@@ -72,7 +72,15 @@ template <class Args> constexpr bool kI8Scan = std::is_base_of<I8Args, Args>::va
 // slice with every tile would cost about twice the code bytes in L2 reads.  The warpgroup widens its own A fragments
 // from the stage's bits and issues m64n32k32.s32.s8.s8 with A in registers.
 struct B1Args : I8Args {};
-template <class Args> constexpr bool kB1Scan = std::is_same<Args, B1Args>::value;
+template <class Args> constexpr bool kB1Scan = std::is_base_of<B1Args, Args>::value;
+
+// Score-all over codes (crag_knn_topk_i8 / _b1): the int8 or one-bit scan's warpgroup and epilogue, so S1 is the same
+// expression bit for bit, and the select warps' ScoreArgs branch, which stores out[q * ld + row].  The constructor
+// leaves ScoreArgs' assignment mode (best_id) off: a running argmax over code rows is not a variant of the scan.
+template <class Codes>
+struct CodeScoreArgs : ScoreArgs, Codes {
+  CodeScoreArgs(float* out, int64_t ld, const Codes& codes) : ScoreArgs{out, ld, nullptr, nullptr, 0}, Codes(codes) {}
+};
 
 // Dynamic shared memory of the scan, from a 1024-byte aligned base: the pipeline stages, (one-bit scan) the resident
 // query block, the score tiles, the selector (select_warps.cuh), then the mbarriers.
@@ -164,7 +172,7 @@ search_topk_kernel(const __grid_constant__ CUtensorMap tm_corpus, const __grid_c
                    uint64_t* __restrict__ pool, uint32_t perm_mul, int perm_shift, uint64_t* __restrict__ part_keys,
                    float* __restrict__ part_minmax, const Args args) {
   constexpr bool IVF = kIvfScan<Args>, SCORES = kScoreScan<Args>, I8 = kI8Scan<Args>, B1 = kB1Scan<Args>;
-  static_assert(!(B1 && (IVF || SCORES)), "the one-bit scan is a flat top-k scan");
+  static_assert(!(B1 && IVF), "the one-bit scan has no IVF variant");
   // elements per 128-byte swizzle row: the producer's column step per k-block
   constexpr int kBlockElems = I8 ? 128 : kBlockK;
   using L = SearchLayout<KLIST, CAP, STAGES, Args>;
@@ -351,10 +359,15 @@ struct SearchPlan {
   size_t total;
 };
 
+// CTAs of a scan: one per SM (132 without a device)
+inline int scan_ctas() {
+  const int g = sm_count();
+  return g > 0 ? g : 132;
+}
+
 SearchPlan plan_search(int k, const void* ws = nullptr) {
   SearchPlan p;
-  p.grid = sm_count();
-  if (p.grid <= 0) p.grid = 132;
+  p.grid = scan_ctas();
   WsCursor c(ws);
   p.part_keys = c.take<uint64_t>(size_t(p.grid) * kNQ * k);
   p.part_minmax = c.take<float>(size_t(p.grid) * kNQ * 2);
@@ -920,37 +933,56 @@ namespace crag {
 namespace {
 inline int64_t knn_ld(int64_t n_rows) { return ((n_rows > 0 ? n_rows : 1) + 3) & ~int64_t(3); }
 
-// Workspace of crag_knn_topk: the fp32 score block [q_chunk][knn_ld(n_rows)]
+// Workspace of crag_knn_topk: the fp32 score block [q_chunk][knn_ld(n_rows)], from byte `at` on (0 for crag_knn_topk,
+// the score-all pass's partials before it for crag_knn_topk_i8 / _b1: knn_code_workspace)
 struct KnnWorkspace { float* block; size_t total; };
-KnnWorkspace knn_workspace(int64_t n_rows, int q_chunk, void* ws = nullptr) {
-  WsCursor c(ws);
+KnnWorkspace knn_workspace(int64_t n_rows, int q_chunk, void* ws = nullptr, size_t at = 0) {
+  WsCursor c(ws, at);
   KnnWorkspace w;
   w.block = c.take<float>(size_t(q_chunk) * size_t(knn_ld(n_rows)));
   w.total = c.bytes;
   return w;
 }
 
-// Per chunk of queries, as many as the workspace holds score rows for: the wgmma GEMM writes the chunk's fp32 score
-// block [nqc, ld] into the workspace (gemm_scores_f32), then `select(q0, nqc, block, ld)` launches its per-query select.
-template <class Select>
-int score_block_chunks(const char* who, const Operand& corpus, const void* queries, int nq, void* workspace,
-                       size_t workspace_bytes, cudaStream_t stream, Select select) {
-  const int64_t ld = knn_ld(corpus.rows);
+// Per chunk of queries, as many as the workspace holds score rows for after its first `at` bytes: `fill(q0, nqc, block,
+// ld)` writes the chunk's fp32 score block [nqc, ld] into the workspace and returns a status, then `select(q0, nqc,
+// block, ld)` launches its per-query select.
+template <class Fill, class Select>
+int score_block_chunks(const char* who, int64_t n_rows, int nq, void* workspace, size_t workspace_bytes, size_t at,
+                       cudaStream_t stream, Fill fill, Select select) {
+  const int64_t ld = knn_ld(n_rows);
   const size_t per_query = size_t(ld) * 4;
-  const size_t fit = workspace_bytes / per_query;
-  if (fit < 1) return fail(CRAG_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes (one query's score row)", who, workspace_bytes, per_query);
+  const size_t fit = workspace_bytes > at ? (workspace_bytes - at) / per_query : 0;
+  if (fit < 1) return fail(CRAG_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes (one query's score row)", who, workspace_bytes, at + per_query);
   const int q_chunk = fit < size_t(nq) ? int(fit) : nq;
-  float* block = knn_workspace(corpus.rows, q_chunk, workspace).block;
-  const int dim = corpus.width;
+  float* block = knn_workspace(n_rows, q_chunk, workspace, at).block;
   for (int q0 = 0; q0 < nq; q0 += q_chunk) {
     const int nqc = (nq - q0) < q_chunk ? (nq - q0) : q_chunk;
-    const int rc = gemm_scores_f32(static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, dim, corpus.ptr, corpus.stride,
-                                   block, ld, nqc, int(corpus.rows), dim, stream);
+    const int rc = fill(q0, nqc, block, ld);
     if (rc != CRAG_OK) return rc;
     select(q0, nqc, block, ld);
     CRAG_CUDA_OK(cudaGetLastError());
   }
   return CRAG_OK;
+}
+
+// The score block of crag_knn_topk and crag_knn_threshold: the wgmma GEMM of a chunk of bf16 queries (gemm_scores_f32)
+auto gemm_fill(const Operand& corpus, const void* queries, cudaStream_t stream) {
+  return [=](int q0, int nqc, float* block, int64_t ld) {
+    const int dim = corpus.width;
+    return gemm_scores_f32(static_cast<const uint8_t*>(queries) + size_t(q0) * dim * 2, dim, corpus.ptr, corpus.stride,
+                           block, ld, nqc, int(corpus.rows), dim, stream);
+  };
+}
+
+// The select of crag_knn_topk and crag_knn_topk_i8 / _b1: knn_select_kernel, one CTA per query of the chunk
+auto knn_select(int64_t n_rows, int k, int64_t row_offset, int64_t* out_ids, float* out_scores, float* out_minmax,
+                cudaStream_t stream) {
+  return [=](int q0, int nqc, const float* block, int64_t ld) {
+    knn_select_kernel<<<nqc, kKnnThreads, 0, stream>>>(block, ld, int(n_rows), k, row_offset, out_ids + size_t(q0) * k,
+                                                       out_scores + size_t(q0) * k,
+                                                       out_minmax ? out_minmax + size_t(q0) * 2 : nullptr);
+  };
 }
 }  // namespace
 }  // namespace crag
@@ -968,12 +1000,8 @@ extern "C" int crag_knn_topk(const void* corpus, int64_t n_rows, int dim, int64_
   int rc = check_scan_args("search", nq, k, kKnnMaxK, c, q, workspace, workspace_bytes, 0);
   if (rc != CRAG_OK) return rc;
   if (!out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "knn: null output pointer");
-  return score_block_chunks("knn", c, queries, nq, workspace, workspace_bytes, stream,
-                            [&](int q0, int nqc, const float* block, int64_t ld) {
-    knn_select_kernel<<<nqc, kKnnThreads, 0, stream>>>(block, ld, int(n_rows), k, row_offset, out_ids + size_t(q0) * k,
-                                                       out_scores + size_t(q0) * k,
-                                                       out_minmax ? out_minmax + size_t(q0) * 2 : nullptr);
-  });
+  return score_block_chunks("knn", n_rows, nq, workspace, workspace_bytes, 0, stream, gemm_fill(c, queries, stream),
+                            knn_select(n_rows, k, row_offset, out_ids, out_scores, out_minmax, stream));
 }
 
 // Threshold join: per chunk of queries the same score block as crag_knn_topk, then knn_threshold_kernel
@@ -993,7 +1021,7 @@ extern "C" int crag_knn_threshold(const void* corpus, int64_t n_rows, int dim, i
     return fail(CRAG_ERR_INVALID, "knn_threshold: need cap >= 1, 0 <= n_exclude <= %d and cap + n_exclude + 1 <= %d (cap=%d n_exclude=%d)",
                 kKnnMaxExclude, kKnnMaxK, cap, n_exclude);
   if (!out_counts || !out_ids || !out_scores || (n_exclude > 0 && !exclude_rows)) return fail(CRAG_ERR_INVALID, "knn_threshold: null pointer");
-  return score_block_chunks("knn_threshold", c, queries, nq, workspace, workspace_bytes, stream,
+  return score_block_chunks("knn_threshold", n_rows, nq, workspace, workspace_bytes, 0, stream, gemm_fill(c, queries, stream),
                             [&](int q0, int nqc, const float* block, int64_t ld) {
     knn_threshold_kernel<<<nqc, kKnnThreads, 0, stream>>>(block, ld, int(n_rows), threshold, limit, cap,
                                                           self_rows ? self_rows + q0 : nullptr, exclude_rows, n_exclude,
@@ -1058,11 +1086,13 @@ __global__ void minmax_reduce_kernel(const float* __restrict__ part_minmax, int 
   }
 }
 
-// Score-all passes (the scan with ScoreArgs), one per block of 32 queries.  Block q0 stores its scores from row q0 of
-// sa.out on, or, in assignment mode (sa.best_id set), updates every row's running argmax with ids counted from q0.
-// out_minmax (may be null) receives each query's (min, max).
-int score_passes(const Operand& corpus, const Operand& queries, ScoreArgs sa, float* out_minmax, const SearchPlan& plan,
-                 cudaStream_t stream) {
+// Score-all passes (the scan with ScoreArgs, or CodeScoreArgs over int8 or one-bit rows), one per block of 32 queries.
+// Block q0 stores its scores from row q0 of sa.out on, or, in assignment mode (sa.best_id set), updates every row's
+// running argmax with ids counted from q0.  out_minmax (may be null) receives each query's (min, max).  Only
+// plan.part_minmax is used.
+template <class Args>
+int score_passes(const Operand& corpus, const Operand& queries, const Args& sa, float* out_minmax,
+                 const SearchPlan& plan, cudaStream_t stream) {
   const int nq = int(queries.rows);
   const int grid = scan_grid(corpus.rows, plan);
   if (grid == 0) {
@@ -1080,10 +1110,11 @@ int score_passes(const Operand& corpus, const Operand& queries, ScoreArgs sa, fl
     CUtensorMap tm_q;
     rc = make_tmap(&tm_q, queries.rows_from(q0, nqc), kNQ);
     if (rc != CRAG_OK) return rc;
-    ScoreArgs pass = sa;
+    Args pass = pass_args(sa, q0);
     if (sa.best_id) pass.base_id = q0;
     else pass.out = sa.out + int64_t(q0) * sa.ld;
-    rc = launch_scan<16, 16, 7>(tm_corpus, tm_q, int(corpus.rows), corpus.num_kb(), nqc, 1, grid, nullptr, nullptr, 0u, 0, nullptr, plan.part_minmax, pass, stream);
+    // k-blocks per row: the queries' 128-byte swizzle rows (a one-bit code row is one box, see scan_pass)
+    rc = launch_scan<16, 16, 7>(tm_corpus, tm_q, int(corpus.rows), queries.num_kb(), nqc, 1, grid, nullptr, nullptr, 0u, 0, nullptr, plan.part_minmax, pass, stream);
     if (rc != CRAG_OK) return rc;
     if (out_minmax) {
       minmax_reduce_kernel<<<nqc, 32, 0, stream>>>(plan.part_minmax, grid, nqc, out_minmax + size_t(q0) * 2);
@@ -1105,6 +1136,66 @@ extern "C" int crag_search_scores(const void* corpus, int64_t n_rows, int dim, i
   if (!out_scores || out_ld < n_rows) return fail(CRAG_ERR_INVALID, "crag_search_scores: need out_scores and out_ld >= n_rows");
   return score_passes(c, q, ScoreArgs{out_scores, out_ld, nullptr, nullptr, 0}, out_minmax, plan,
                       static_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------ exact top-k up to 2048 over int8 and one-bit codes
+namespace crag {
+namespace {
+// Workspace of crag_knn_topk_i8 / _b1: the score-all pass's per-CTA (min, max) (all of a SearchPlan that score_passes
+// reads), then the score block (knn_workspace from the end of these partials on)
+SearchPlan plan_score_parts(const void* ws = nullptr) {
+  SearchPlan p{};
+  p.grid = scan_ctas();
+  WsCursor c(ws);
+  p.part_minmax = c.take<float>(size_t(p.grid) * kNQ * 2);
+  p.parts_bytes = p.total = c.bytes;
+  return p;
+}
+
+// Per chunk of queries the score-all passes over the codes write the chunk's S1 block, then crag_knn_topk's select
+// keeps each query's k best rows.
+template <class Codes>
+int knn_code_topk(const char* who, const Operand& corpus, const Operand& queries, const Codes& codes, int64_t row_offset,
+                  int k, int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace, size_t workspace_bytes,
+                  cudaStream_t stream) {
+  const SearchPlan parts = plan_score_parts(workspace);
+  return score_block_chunks(who, corpus.rows, int(queries.rows), workspace, workspace_bytes, parts.total, stream,
+                            [&](int q0, int nqc, float* block, int64_t ld) {
+                              const CodeScoreArgs<Codes> sa(block, ld, codes);
+                              return score_passes(corpus, queries.rows_from(q0, nqc), pass_args(sa, q0), nullptr, parts, stream);
+                            },
+                            knn_select(corpus.rows, k, row_offset, out_ids, out_scores, out_minmax, stream));
+}
+}  // namespace
+}  // namespace crag
+
+extern "C" size_t crag_knn_code_workspace_bytes(int64_t n_rows, int q_chunk) {
+  if (n_rows < 0 || q_chunk < 1) return 0;
+  return knn_workspace(n_rows, q_chunk, nullptr, plan_score_parts().total).total;
+}
+
+extern "C" int crag_knn_topk_i8(const void* codes, const float* row_scales, int64_t n_rows, int dim8, int64_t row_stride,
+                                int64_t row_offset, const void* queries_i8, const float* query_scales, int nq, int k,
+                                int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                                size_t workspace_bytes, crag_stream_t stream) {
+  const Operand c{codes, n_rows, dim8, row_stride, kS8, "corpus"}, q{queries_i8, nq, dim8, dim8, kS8, "queries"};
+  int rc = check_scan_args("search_i8", nq, k, kKnnMaxK, c, q, workspace, workspace_bytes, plan_score_parts().total);
+  if (rc != CRAG_OK) return rc;
+  if (!query_scales || !out_ids || !out_scores || (n_rows > 0 && !row_scales)) return fail(CRAG_ERR_INVALID, "search_i8: null pointer");
+  return knn_code_topk("knn_i8", c, q, I8Args{row_scales, query_scales}, row_offset, k, out_ids, out_scores, out_minmax,
+                       workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int crag_knn_topk_b1(const void* bits, const float* alpha, int64_t n_rows, int dim8, int64_t row_stride,
+                                int64_t row_offset, const void* queries_i8, const float* query_scales, int nq, int k,
+                                int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                                size_t workspace_bytes, crag_stream_t stream) {
+  const Operand c{bits, n_rows, dim8 / 8, row_stride, kS8, "bits", true}, q{queries_i8, nq, dim8, dim8, kS8, "queries_i8"};
+  int rc = check_scan_args("search_b1", nq, k, kKnnMaxK, c, q, workspace, workspace_bytes, plan_score_parts().total);
+  if (rc != CRAG_OK) return rc;
+  if ((n_rows > 0 && !alpha) || !query_scales || !out_ids || !out_scores) return fail(CRAG_ERR_INVALID, "search_b1: null alpha, query_scales or output pointer");
+  return knn_code_topk("knn_b1", c, q, B1Args{{alpha, query_scales}}, row_offset, k, out_ids, out_scores, out_minmax,
+                       workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------ fused finalize + exchange (row-sharded index)

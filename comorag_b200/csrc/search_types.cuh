@@ -77,7 +77,7 @@ struct ScoreArgs {
 // A scan variant is named by its argument struct; the select warps take it as the flags IVF / SCORES, which IvfParam
 // maps back to a bf16 variant's struct (tests/warp_emu/select_shell.h).
 template <class Args> constexpr bool kIvfScan = std::is_base_of<IvfArgs, Args>::value;
-template <class Args> constexpr bool kScoreScan = std::is_same<Args, ScoreArgs>::value;
+template <class Args> constexpr bool kScoreScan = std::is_base_of<ScoreArgs, Args>::value;
 template <bool IVF, bool SCORES> struct IvfParam { using type = NoIvfArgs; };
 template <> struct IvfParam<true, false> { using type = IvfArgs; };
 template <> struct IvfParam<false, true> { using type = ScoreArgs; };

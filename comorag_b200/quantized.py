@@ -1,7 +1,8 @@
 """Int8 snapshot of a DenseIndex: a scan that reads half the bytes of the bf16 shard, then an exact bf16 rescore.
 
 A search runs crag_search_topk_i8 over the int8 rows for `candidates` rows per query, then crag_rescore_topk
-recomputes each candidate's score from its bf16 row and the bf16 query and keeps the best k.  The returned scores are
+recomputes each candidate's score from its bf16 row and the bf16 query and keeps the best k.  search_wide takes up to
+2048 candidates: above 128 its stage 1 is crag_knn_topk_i8, a score-all pass over the codes and a per-query select.  The returned scores are
 those exact fp32 dots; only the choice of candidates comes from the int8 scores.  The bf16 rows are read for the
 candidates only, so they may live in page-locked host memory (rows="host"), which halves the device footprint again.
 Semantics: DESIGN.md section 3e and oracle/quant_oracle.py.
@@ -14,7 +15,7 @@ import numpy as np
 import torch
 
 from . import _native
-from .index import MAX_K, DenseIndex
+from .index import KNN_MAX_K, MAX_K, DenseIndex, knn_chunk
 
 
 def _dim8(dim: int) -> int:
@@ -79,8 +80,8 @@ def rescored_candidates(k: int, candidates: Optional[int]) -> int:
 class QuantizedIndex:
     """Frozen int8 snapshot of a DenseIndex's rows (rows added to the DenseIndex later are not seen).
 
-    A subclass with another row code (binary.BinaryIndex) overrides _encode and _scan; the snapshot, the query checks
-    and the rescore are shared."""
+    A subclass with another row code (binary.BinaryIndex) overrides _encode and _stage1; the snapshot, the query
+    checks and the rescore are shared."""
 
     def __init__(self, rows_bf16: torch.Tensor, codes: torch.Tensor, scales: torch.Tensor, dim: int,
                  device: torch.device, row_offset: int):
@@ -98,15 +99,22 @@ class QuantizedIndex:
         """(code rows, per-row scales) of device bf16 rows."""
         return quantize_rows(rows, dim8)
 
+    @staticmethod
+    def _stage1(wide: bool) -> str:
+        """The C entry of stage 1 over this class's codes: the top-k scan (<= 128 candidates) or, wide, the score-all
+        pass and per-query select (<= 2048).  Both take the same arguments."""
+        return "crag_knn_topk_i8" if wide else "crag_search_topk_i8"
+
     def _scan(self, q8: torch.Tensor, qs: torch.Tensor, candidates: int, c_ids: torch.Tensor, c_sc: torch.Tensor,
-              ws: torch.Tensor, st: torch.cuda.Stream) -> None:
+              ws: torch.Tensor, st: torch.cuda.Stream, wide: bool) -> None:
         """Stage 1: the top `candidates` rows of every query into (c_ids, c_sc)."""
         n, nq = self.n_rows, q8.shape[0]
-        rc = _native.load().crag_search_topk_i8(self._codes.data_ptr() if n else 0, self._scales.data_ptr() if n else 0,
-                                                n, self.dim8, self.dim8, self.row_offset, q8.data_ptr(), qs.data_ptr(),
-                                                nq, candidates, c_ids.data_ptr(), c_sc.data_ptr(), 0, ws.data_ptr(),
-                                                ws.numel(), st.cuda_stream)
-        _native.check(rc, "crag_search_topk_i8")
+        name = self._stage1(wide)
+        rc = getattr(_native.load(), name)(self._codes.data_ptr() if n else 0, self._scales.data_ptr() if n else 0, n,
+                                           self.dim8, self._codes.shape[1], self.row_offset, q8.data_ptr(),
+                                           qs.data_ptr(), nq, candidates, c_ids.data_ptr(), c_sc.data_ptr(), 0,
+                                           ws.data_ptr(), ws.numel(), st.cuda_stream)
+        _native.check(rc, name)
 
     @classmethod
     def from_dense(cls, index: DenseIndex, rows: str = "device") -> "QuantizedIndex":
@@ -145,7 +153,21 @@ class QuantizedIndex:
         """Top k of a device bf16 [nq, dim_pad] query block: (ids int64 [nq, k], scores fp32 [nq, k]) on the device.
         Scores are the exact fp32 dots of the rescore (descending, ties by ascending id); -1 / -inf where fewer than
         k rows exist.  candidates (default min(128, 4 k)) rows per query come from the scan of the code rows."""
-        candidates = rescored_candidates(k, candidates)
+        return self._search_device(queries, k, rescored_candidates(k, candidates), stream, wide=False)
+
+    def search_device_wide(self, queries: torch.Tensor, k: int, candidates: int,
+                           stream: Optional[torch.cuda.Stream] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """search_device for up to 2048 candidates (1 <= k <= candidates <= 2048): at most 128 it is search_device;
+        above, stage 1 is the exact top `candidates` of every row's code score (crag_knn_topk_i8 / _b1, per chunk of
+        queries whose score rows fit index.knn_chunk's budget), and the rescore sorts them all."""
+        if not 1 <= k <= candidates <= KNN_MAX_K:
+            raise ValueError(f"need 1 <= k <= candidates <= {KNN_MAX_K} (k={k}, candidates={candidates})")
+        if candidates <= MAX_K:
+            return self.search_device(queries, k, candidates, stream)
+        return self._search_device(queries, k, candidates, stream, wide=True)
+
+    def _search_device(self, queries: torch.Tensor, k: int, candidates: int, stream: Optional[torch.cuda.Stream],
+                       wide: bool) -> Tuple[torch.Tensor, torch.Tensor]:
         if queries.dtype != torch.bfloat16 or queries.dim() != 2 or queries.shape[1] != self.dim_pad or not queries.is_cuda:
             raise ValueError(f"queries must be device bf16 [nq, {self.dim_pad}]")
         queries = queries.contiguous()
@@ -159,9 +181,12 @@ class QuantizedIndex:
                 q8, qs = quantize_rows(queries, self.dim8, st)
                 c_ids = torch.empty((nq, candidates), dtype=torch.int64, device=dev)
                 c_sc = torch.empty((nq, candidates), dtype=torch.float32, device=dev)
-                ws_bytes = lib.crag_search_workspace_bytes(nq, candidates)
+                if wide:
+                    ws_bytes = lib.crag_knn_code_workspace_bytes(n, knn_chunk(nq, n))
+                else:
+                    ws_bytes = lib.crag_search_workspace_bytes(nq, candidates)
                 ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-                self._scan(q8, qs, candidates, c_ids, c_sc, ws, st)
+                self._scan(q8, qs, candidates, c_ids, c_sc, ws, st, wide)
                 ids = torch.empty((nq, k), dtype=torch.int64, device=dev)
                 scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
                 rc = lib.crag_rescore_topk(self._rows.data_ptr() if n else 0, n, self.dim_pad,
@@ -175,4 +200,11 @@ class QuantizedIndex:
         """Host entry point: what DenseIndex.prepare_queries accepts in, numpy (ids int64 [nq, k], scores fp32
         [nq, k]) out."""
         ids, scores = self.search_device(self.prepare_queries(queries), k, candidates)
+        return ids.cpu().numpy(), scores.cpu().numpy()
+
+    def search_wide(self, queries, k: int, candidates: int) -> Tuple[np.ndarray, np.ndarray]:
+        """search_device_wide's host twin, as search is search_device's."""
+        if not 1 <= k <= candidates <= KNN_MAX_K:
+            raise ValueError(f"need 1 <= k <= candidates <= {KNN_MAX_K} (k={k}, candidates={candidates})")
+        ids, scores = self.search_device_wide(self.prepare_queries(queries), k, candidates)
         return ids.cpu().numpy(), scores.cpu().numpy()

@@ -129,7 +129,7 @@ CRAG_API int crag_search_topk_i8(const void* corpus_i8, const float* row_scales,
                                  int64_t row_stride, int64_t row_offset, const void* queries_i8,
                                  const float* query_scales, int nq, int k, int64_t* out_ids, float* out_scores,
                                  float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream);
-/* crag_rescore_topk: per query, the top k (1 <= k <= n_cand <= 128) of its n_cand candidates cand_ids (device int64
+/* crag_rescore_topk: per query, the top k (1 <= k <= n_cand <= 2048) of its n_cand candidates cand_ids (device int64
  * [nq, n_cand], global ids) by the fp32 dot of the bf16 row and the bf16 query, summed in the pinned order of DESIGN.md
  * section 3e; ties by ascending row; -1 / -inf past the valid candidates.  An id outside [row_offset, row_offset +
  * n_rows) is no candidate (as -1) and its row is never read.
@@ -167,6 +167,25 @@ CRAG_API int crag_search_topk_b1(const void* bits, const float* alpha, int64_t n
                                  int64_t row_offset, const void* queries_i8, const float* query_scales, int nq, int k,
                                  int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
                                  size_t workspace_bytes, crag_stream_t stream);
+
+/* Candidates beyond 128 for int8 and one-bit shards (DESIGN.md section 3f): the exact top k, 1 <= k <= 2048, of the
+ * same S1 as crag_search_topk_i8 / crag_search_topk_b1, with their operand rules and error messages.  Per chunk of
+ * queries the scan's score-all pass writes every row's S1 into a fp32 block [q_chunk, round_up(n_rows, 4)] of the
+ * workspace, then one CTA per query radix-selects its k best, as crag_knn_topk does.  Ties by ascending row, -1 / -inf
+ * past n_rows; out_minmax (may be null) is the (min, max) of S1 over all rows, (+inf, -inf) for an empty shard.
+ * crag_knn_code_workspace_bytes(n_rows, q) is the size that holds the score-all pass's per-CTA partials and q
+ * queries' score rows; q_chunk is as many rows as a given workspace holds after the partials (>= 1, else
+ * CRAG_ERR_WORKSPACE).  Workspace 256-B aligned.  Feeding the candidates to crag_rescore_topk gives the exact bf16
+ * answer over up to 2048 candidates per query. */
+CRAG_API size_t crag_knn_code_workspace_bytes(int64_t n_rows, int q_chunk);
+CRAG_API int crag_knn_topk_i8(const void* codes, const float* row_scales, int64_t n_rows, int dim8, int64_t row_stride,
+                              int64_t row_offset, const void* queries_i8, const float* query_scales, int nq, int k,
+                              int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                              size_t workspace_bytes, crag_stream_t stream);
+CRAG_API int crag_knn_topk_b1(const void* bits, const float* alpha, int64_t n_rows, int dim8, int64_t row_stride,
+                              int64_t row_offset, const void* queries_i8, const float* query_scales, int nq, int k,
+                              int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
+                              size_t workspace_bytes, crag_stream_t stream);
 
 /* Exact top-k for large k and/or many queries: per chunk of queries one wgmma GEMM writes the fp32 score block
  * [q_chunk, round_up(n_rows, 4)] into the workspace, then one CTA per query radix-selects its k best.
