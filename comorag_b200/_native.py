@@ -114,6 +114,17 @@ SIGNATURES = {
                                      C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,
                                      C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "crag_ivf_i8_wide_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int, C.c_int64]),
+    "crag_ivf_search_i8_wide": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int64,
+                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                          C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                          C.c_void_p]),
+    "crag_ivf_pq_wide_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int]),
+    "crag_ivf_search_pq_wide": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
+                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,
+                                          C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "crag_pq_encode": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
                                  C.c_void_p]),
     "crag_gmm_sweep_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),

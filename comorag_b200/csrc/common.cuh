@@ -58,7 +58,8 @@ int check_workspace(const char* who, const void* ws, size_t bytes, size_t need);
 // quant.cu.  The address a kernel reads `p` through: device memory as is, page-locked host memory through its device
 // mapping; anything else (pageable host memory) fails with CRAG_ERR_INVALID, `who` heading the message.
 int device_readable(const void* p, const void** out, const char* who);
-// quant.cu: ivf_rescore_topk_kernel (quant_kernels.cuh) for one 32-query pass of crag_ivf_search_i8
+// quant.cu: the IVF rescore (quant_kernels.cuh) of one 32-query pass of the rescored IVF searches:
+// ivf_rescore_topk_kernel up to 128 candidates, ivf_rescore_wide_kernel up to 2048
 int launch_ivf_rescore(const void* rows, int64_t n_rows, int dim, int64_t row_stride, const void* queries, int nq,
                        const int64_t* cand, int n_cand, int k, const int32_t* list_tile_start, int nlist,
                        const float* coarse, int64_t* out_ids, float* out_scores, cudaStream_t stream);

@@ -12,46 +12,12 @@
 //   3. bitonic sort of the <= 2048 collected keys in shared memory (16 KB, knn_sort.cuh), ids row + row_offset out.
 // (min, max) over all rows is reduced in the gather pass.  n_rows <= k skips step 1 and sorts every row.
 // Pure SIMT code with no wgmma / TMA / mbarrier in it, so tests/warp_emu runs this very header on emulated blocks.
-#pragma once
-#include <stdint.h>
-#include <cuda_runtime.h>
-
-#include "knn_sort.cuh"
-#include "topk.cuh"
-
-namespace crag {
-namespace {
-
-constexpr int kKnnBins = 2048;
-constexpr int kKnnLoads = 4;   // 16-byte loads per thread in flight in a histogram pass
-
-// Exclusive scan of v over the block's threads in threadIdx order; *total = the sum over all threads.
-__device__ __forceinline__ int knn_block_exclusive_scan(int v, int* s_warp, int* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_sync(0xffffffffu, x, lane >= o ? lane - o : lane);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) s_warp[warp] = x;
-  __syncthreads();
-  int before = 0, all = 0;
-#pragma unroll
-  for (int w = 0; w < kKnnWarps; ++w) {
-    const int c = s_warp[w];
-    before += w < warp ? c : 0;
-    all += c;
-  }
-  __syncthreads();   // s_warp is free for the next call
-  *total = all;
-  return before + x - v;
-}
-
-// scores: fp32 rows of `ld` floats (ld % 4 == 0, 16-byte aligned), block q reads row q; outputs [gridDim.x, k].
-__global__ void __launch_bounds__(kKnnThreads)
-knn_select_kernel(const float* __restrict__ scores, int64_t ld, int n_rows, int k, int64_t row_offset,
-                  int64_t* __restrict__ out_ids, float* __restrict__ out_scores, float* __restrict__ out_minmax) {
+// This file is also the body of the select kernels: each includes it with CRAG_KNN_SELECT_BODY defined and gets the
+// text of the select (the #if branch below), which reads the names the kernel declares -- scores, ld, n_rows, k,
+// row_offset, out_ids, out_scores, out_minmax -- and selects for block q = blockIdx.x.  It is text rather than a device
+// function because wrapping it in one, even inlined, changes knn_select_kernel's SASS: nvcc optimises the callee
+// before inlining it.
+#if defined(CRAG_KNN_SELECT_BODY)
   __shared__ uint32_t s_hist[kKnnBins];
   __shared__ uint64_t s_keys[kKnnMaxK];
   __shared__ int s_warp[kKnnWarps];
@@ -205,7 +171,65 @@ knn_select_kernel(const float* __restrict__ scores, int64_t ld, int n_rows, int 
     out_minmax[int64_t(q) * 2 + 0] = n_rows > 0 ? unorderable_f32(a) : INFINITY;
     out_minmax[int64_t(q) * 2 + 1] = n_rows > 0 ? unorderable_f32(b) : -INFINITY;
   }
+#elif !defined(CRAG_KNN_SELECT_CUH)
+#define CRAG_KNN_SELECT_CUH
+#include <stdint.h>
+#include <cuda_runtime.h>
+
+#include "knn_sort.cuh"
+#include "topk.cuh"
+
+namespace crag {
+namespace {
+
+constexpr int kKnnBins = 2048;
+constexpr int kKnnLoads = 4;   // 16-byte loads per thread in flight in a histogram pass
+
+// Exclusive scan of v over the block's threads in threadIdx order; *total = the sum over all threads.
+__device__ __forceinline__ int knn_block_exclusive_scan(int v, int* s_warp, int* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_sync(0xffffffffu, x, lane >= o ? lane - o : lane);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) s_warp[warp] = x;
+  __syncthreads();
+  int before = 0, all = 0;
+#pragma unroll
+  for (int w = 0; w < kKnnWarps; ++w) {
+    const int c = s_warp[w];
+    before += w < warp ? c : 0;
+    all += c;
+  }
+  __syncthreads();   // s_warp is free for the next call
+  *total = all;
+  return before + x - v;
+}
+
+// scores: fp32 rows of `ld` floats (ld % 4 == 0, 16-byte aligned), block q reads row q; outputs [gridDim.x, k].
+__global__ void __launch_bounds__(kKnnThreads)
+knn_select_kernel(const float* __restrict__ scores, int64_t ld, int n_rows, int k, int64_t row_offset,
+                  int64_t* __restrict__ out_ids, float* __restrict__ out_scores, float* __restrict__ out_minmax) {
+#define CRAG_KNN_SELECT_BODY
+#include "knn_select.cuh"
+#undef CRAG_KNN_SELECT_BODY
+}
+
+// The ragged select of the wide IVF stage 1 (crag_ivf_search_i8_wide / _pq_wide): block q ranks the first n_q[q] slots
+// of row q of the pass's S1 block (ivf_wide_plan_kernel's row counts) and writes slot ids, which ivf_slot_map_kernel
+// turns into stored positions.
+__global__ void __launch_bounds__(kKnnThreads)
+ivf_wide_select_kernel(const float* __restrict__ scores, int64_t ld, const int32_t* __restrict__ n_q, int k,
+                       int64_t* __restrict__ out_ids, float* __restrict__ out_scores, float* __restrict__ out_minmax) {
+  const int n_rows = __ldg(&n_q[blockIdx.x]);
+  const int64_t row_offset = 0;
+#define CRAG_KNN_SELECT_BODY
+#include "knn_select.cuh"
+#undef CRAG_KNN_SELECT_BODY
 }
 
 }  // namespace
 }  // namespace crag
+#endif

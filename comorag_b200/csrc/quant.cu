@@ -31,9 +31,13 @@ int device_readable(const void* p, const void** out, const char* who) {
 int launch_ivf_rescore(const void* rows, int64_t n_rows, int dim, int64_t row_stride, const void* queries, int nq,
                        const int64_t* cand, int n_cand, int k, const int32_t* list_tile_start, int nlist,
                        const float* coarse, int64_t* out_ids, float* out_scores, cudaStream_t stream) {
-  ivf_rescore_topk_kernel<<<nq, kRescoreThreads, 0, stream>>>(
-      static_cast<const uint16_t*>(rows), n_rows, dim, row_stride, static_cast<const uint16_t*>(queries), cand, n_cand, k,
-      out_ids, out_scores, IvfListTerm{list_tile_start, nlist, coarse});
+  const IvfListTerm lists{list_tile_start, nlist, coarse};
+  const uint16_t* r = static_cast<const uint16_t*>(rows);
+  const uint16_t* qb = static_cast<const uint16_t*>(queries);
+  if (n_cand <= kRescoreMaxCand)   // one warp sorts the keys in registers
+    ivf_rescore_topk_kernel<<<nq, kRescoreThreads, 0, stream>>>(r, n_rows, dim, row_stride, qb, cand, n_cand, k, out_ids, out_scores, lists);
+  else                             // a block sorts them in shared memory (crag_ivf_search_i8_wide / _pq_wide)
+    ivf_rescore_wide_kernel<<<nq, kKnnThreads, 0, stream>>>(r, n_rows, dim, row_stride, qb, cand, n_cand, k, out_ids, out_scores, lists);
   CRAG_CUDA_OK(cudaGetLastError());
   return CRAG_OK;
 }

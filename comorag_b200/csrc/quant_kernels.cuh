@@ -215,19 +215,22 @@ ivf_rescore_topk_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int d
   rescore_topk_body(rows, n_rows, dim, row_stride, int64_t(0), queries, cand_ids, n_cand, k, out_ids, out_scores, lists);
 }
 
-// crag_rescore_topk above 128 candidates (n_cand <= kKnnMaxK): one CTA of kKnnThreads per query, one warp per candidate
-// (rescore_key, as rescore_topk_kernel computes it), the keys in shared memory (16 KB at 2048) sorted by
-// knn_bitonic_sort, the top k out; -1 / -inf past the valid candidates.
-__global__ void __launch_bounds__(kKnnThreads)
-rescore_wide_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride, int64_t row_offset,
-                    const uint16_t* __restrict__ queries, const int64_t* __restrict__ cand_ids, int n_cand, int k,
-                    int64_t* __restrict__ out_ids, float* __restrict__ out_scores) {
+// The body of both wide rescore kernels, above 128 candidates (n_cand <= kKnnMaxK): one CTA of kKnnThreads per query,
+// one warp per candidate (rescore_key, as rescore_topk_body computes it), the keys in shared memory (16 KB at 2048)
+// sorted by knn_bitonic_sort, the top k out; -1 / -inf past the valid candidates.
+template <class ListTerm>
+__device__ __forceinline__ void rescore_wide_body(const uint16_t* __restrict__ rows, int64_t n_rows, int dim,
+                                                  int64_t row_stride, int64_t row_offset,
+                                                  const uint16_t* __restrict__ queries,
+                                                  const int64_t* __restrict__ cand_ids, int n_cand, int k,
+                                                  int64_t* __restrict__ out_ids, float* __restrict__ out_scores,
+                                                  const ListTerm& lists) {
   __shared__ uint64_t s_keys[kKnnMaxK];
   const int q = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint16_t* qv = queries + int64_t(q) * dim;
   const int64_t* cand = cand_ids + int64_t(q) * n_cand;
   for (int c = warp; c < n_cand; c += kKnnWarps) {
-    const uint64_t key = rescore_key(rows, n_rows, dim / 8, row_stride, qv, __ldg(&cand[c]) - row_offset, q, lane, NoListTerm{});
+    const uint64_t key = rescore_key(rows, n_rows, dim / 8, row_stride, qv, __ldg(&cand[c]) - row_offset, q, lane, lists);
     if (lane == 0) s_keys[c] = key;
   }
   knn_bitonic_sort(s_keys, n_cand, tid);
@@ -236,6 +239,23 @@ rescore_wide_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, 
     out_ids[int64_t(q) * k + j] = key ? int64_t(key_id(key)) + row_offset : -1;
     out_scores[int64_t(q) * k + j] = key ? key_score(key) : -INFINITY;
   }
+}
+
+// crag_rescore_topk above 128 candidates
+__global__ void __launch_bounds__(kKnnThreads)
+rescore_wide_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride, int64_t row_offset,
+                    const uint16_t* __restrict__ queries, const int64_t* __restrict__ cand_ids, int n_cand, int k,
+                    int64_t* __restrict__ out_ids, float* __restrict__ out_scores) {
+  rescore_wide_body(rows, n_rows, dim, row_stride, row_offset, queries, cand_ids, n_cand, k, out_ids, out_scores, NoListTerm{});
+}
+
+// crag_ivf_search_i8_wide / _pq_wide, one 32-query pass: up to 2048 candidate positions per query, as
+// ivf_rescore_topk_kernel scores them
+__global__ void __launch_bounds__(kKnnThreads)
+ivf_rescore_wide_kernel(const uint16_t* __restrict__ rows, int64_t n_rows, int dim, int64_t row_stride,
+                        const uint16_t* __restrict__ queries, const int64_t* __restrict__ cand_ids, int n_cand, int k,
+                        int64_t* __restrict__ out_ids, float* __restrict__ out_scores, const IvfListTerm lists) {
+  rescore_wide_body(rows, n_rows, dim, row_stride, int64_t(0), queries, cand_ids, n_cand, k, out_ids, out_scores, lists);
 }
 
 }  // namespace crag

@@ -34,7 +34,8 @@
 // top-k up to k = 2048 for large query batches as a score-block GEMM (gemm.cu)
 // plus a per-query radix select (knn_select.cuh), and crag_knn_threshold -- the same score block, then a per-query
 // threshold join (knn_threshold.cuh).  crag_ivf_search_pq runs the IVF plan, then the PQ table and scan kernels
-// (pq_kernels.cuh), then the same merge, rescore and id map as crag_ivf_search_i8.
+// (pq_kernels.cuh), then the same merge, rescore and id map as crag_ivf_search_i8.  Their _wide forms score every
+// probed row into a block (ivf_wide_kernels.cuh) and radix-select up to 2048 candidates per query.
 #include <algorithm>
 #include <type_traits>
 
@@ -50,6 +51,7 @@
 #include "knn_select.cuh"
 #include "knn_threshold.cuh"
 #include "pq_kernels.cuh"
+#include "ivf_wide_kernels.cuh"
 #include "binary.cuh"
 #include "workspace.cuh"
 
@@ -608,40 +610,48 @@ struct IvfRescore {
   float* cand_scores;
 };
 
-// Every 32-query pass of an IVF search: the plan of the probed tiles, stage 1 for n_scan keys per query, the merge of
-// its partials, then the map of stored positions to original ids.  `stage1(q0, nqc, parts)` launches stage 1 for
-// queries q0 .. q0 + nqc - 1 and sets `parts` to the number of partial lists it wrote.  With `rescore` the merge writes
-// n_scan candidates, which the exact rescore (quant.cu) turns into the k results, with the plan's coarse terms.
-template <class Stage1>
-int ivf_passes(int nq, const IvfLists& l, int n_scan, int k, const IvfRescore* rescore, int64_t* out_ids,
-               float* out_scores, float* out_minmax, const IvfPlan& ip, cudaStream_t stream, Stage1 stage1) {
-  const SearchPlan& sp = ip.scan;
+// Every 32-query pass of an IVF search: the plan of the probed tiles, then `fine(q0, nqc, ids, scores, minmax)`, which
+// writes the k results of queries q0 .. q0 + nqc - 1 as stored positions into the outputs it is given, then the map of
+// stored positions to original ids.
+template <class Fine>
+int ivf_pass_loop(int nq, const IvfLists& l, int k, int64_t* out_ids, float* out_scores, float* out_minmax,
+                  const IvfPlan& ip, cudaStream_t stream, Fine fine) {
   for (int q0 = 0; q0 < nq; q0 += kNQ) {
     const int nqc = (nq - q0) < kNQ ? (nq - q0) : kNQ;
     ivf_plan_kernel<<<1, 1024, 0, stream>>>(l.probed_ids + size_t(q0) * l.nprobe, l.probed_scores + size_t(q0) * l.nprobe, nqc,
                                             l.nprobe, l.nlist, l.tile_start, l.rows, ip.list_mask, ip.coarse, ip.work,
                                             ip.n_work);
     CRAG_CUDA_OK(cudaGetLastError());
-    int parts = 0;
-    int rc = stage1(q0, nqc, parts);
-    if (rc != CRAG_OK) return rc;
     int64_t* ids = out_ids + size_t(q0) * k;
-    float* scores = out_scores + size_t(q0) * k;
-    float* minmax = out_minmax ? out_minmax + size_t(q0) * 2 : nullptr;
-    if (!rescore) {
-      rc = finalize_parts(parts, nqc, k, 0, ids, scores, minmax, nullptr, sp, stream);
-    } else {
-      rc = finalize_parts(parts, nqc, n_scan, 0, rescore->cand_ids, rescore->cand_scores, minmax, nullptr, sp, stream);
-      if (rc == CRAG_OK)
-        rc = launch_ivf_rescore(rescore->rows.ptr, rescore->rows.rows, rescore->rows.width, rescore->rows.stride,
-                                rescore->queries.rows_from(q0, nqc).ptr, nqc, rescore->cand_ids, n_scan, k, l.tile_start,
-                                l.nlist, ip.coarse, ids, scores, stream);
-    }
+    const int rc = fine(q0, nqc, ids, out_scores + size_t(q0) * k, out_minmax ? out_minmax + size_t(q0) * 2 : nullptr);
     if (rc != CRAG_OK) return rc;
     ivf_map_ids_kernel<<<(nqc * k + 255) / 256, 256, 0, stream>>>(ids, nqc * k, l.row_ids);
     CRAG_CUDA_OK(cudaGetLastError());
   }
   return CRAG_OK;
+}
+
+// The passes of an IVF search whose stage 1 keeps n_scan keys per query in per-CTA partial lists.
+// `stage1(q0, nqc, parts)` launches stage 1 for queries q0 .. q0 + nqc - 1 and sets `parts` to the number of partial
+// lists it wrote.  With `rescore` the merge writes n_scan candidates, which the exact rescore (quant.cu) turns into the
+// k results, with the plan's coarse terms.
+template <class Stage1>
+int ivf_passes(int nq, const IvfLists& l, int n_scan, int k, const IvfRescore* rescore, int64_t* out_ids,
+               float* out_scores, float* out_minmax, const IvfPlan& ip, cudaStream_t stream, Stage1 stage1) {
+  const SearchPlan& sp = ip.scan;
+  return ivf_pass_loop(nq, l, k, out_ids, out_scores, out_minmax, ip, stream,
+                       [&](int q0, int nqc, int64_t* ids, float* scores, float* minmax) {
+    int parts = 0;
+    int rc = stage1(q0, nqc, parts);
+    if (rc != CRAG_OK) return rc;
+    if (!rescore) return finalize_parts(parts, nqc, k, 0, ids, scores, minmax, nullptr, sp, stream);
+    rc = finalize_parts(parts, nqc, n_scan, 0, rescore->cand_ids, rescore->cand_scores, minmax, nullptr, sp, stream);
+    if (rc == CRAG_OK)
+      rc = launch_ivf_rescore(rescore->rows.ptr, rescore->rows.rows, rescore->rows.width, rescore->rows.stride,
+                              rescore->queries.rows_from(q0, nqc).ptr, nqc, rescore->cand_ids, n_scan, k, l.tile_start,
+                              l.nlist, ip.coarse, ids, scores, stream);
+    return rc;
+  });
 }
 
 // The IVF passes whose stage 1 is the scan of the probed tiles of the residuals `res` (bf16 or int8, as Args says).
@@ -667,25 +677,26 @@ int ivf_scan_passes(const Operand& res, const Operand& queries, Args args, const
                     });
 }
 
-// The argument rules of the rescored IVF searches (crag_ivf_search_i8, crag_ivf_search_pq): the lists, probes and
-// outputs, nq >= 1 and 1 <= k <= n_cand <= 128, then the entry's own rules (`entry_check()`), the bf16 residuals and
-// queries of the rescore, and a workspace of `need` bytes.  Then points r.rows at the device address of the bf16
-// residuals, which may be page-locked host memory (pageable memory is refused before any launch), and r's candidates
-// at `cand`'s buffers.
+// The argument rules of the rescored IVF searches (crag_ivf_search_i8 / _pq and their _wide forms): the lists, probes
+// and outputs, nq >= 1 and 1 <= k <= n_cand <= max_cand (128, or 2048 for the wide forms), then the entry's own rules
+// (`entry_check()`), the bf16 residuals and queries of the rescore, and a workspace of `need` bytes.  Then points
+// r.rows at the device address of the bf16 residuals, which may be page-locked host memory (pageable memory is refused
+// before any launch), and r's candidates at the workspace's buffers `cand_ids` / `cand_scores`.
 template <class EntryCheck>
-int check_rescored_ivf(const char* who, const IvfLists& l, int64_t n_rows_padded, int nq, int n_cand, int k,
-                       const int64_t* out_ids, const float* out_scores, IvfRescore& r, const IvfI8Plan& cand,
-                       const void* workspace, size_t workspace_bytes, size_t need, EntryCheck entry_check) {
+int check_rescored_ivf(const char* who, const IvfLists& l, int64_t n_rows_padded, int nq, int n_cand, int k, int max_cand,
+                       const int64_t* out_ids, const float* out_scores, IvfRescore& r, int64_t* cand_ids,
+                       float* cand_scores, const void* workspace, size_t workspace_bytes, size_t need,
+                       EntryCheck entry_check) {
   int rc = check_ivf_args(who, l, n_rows_padded, out_ids, out_scores);
   if (rc != CRAG_OK) return rc;
-  if (nq < 1 || k < 1 || n_cand < k || n_cand > 128) return fail(CRAG_ERR_INVALID, "%s: need nq >= 1 and 1 <= k <= n_cand <= 128 (nq=%d k=%d n_cand=%d)", who, nq, k, n_cand);
+  if (nq < 1 || k < 1 || n_cand < k || n_cand > max_cand) return fail(CRAG_ERR_INVALID, "%s: need nq >= 1 and 1 <= k <= n_cand <= %d (nq=%d k=%d n_cand=%d)", who, max_cand, nq, k, n_cand);
   rc = entry_check();
   if (rc == CRAG_OK) rc = check_operand(who, r.rows);
   if (rc == CRAG_OK) rc = check_operand(who, r.queries);
   if (rc == CRAG_OK) rc = check_workspace(who, workspace, workspace_bytes, need);
   if (rc == CRAG_OK) rc = device_readable(r.rows.ptr, &r.rows.ptr, who);
-  r.cand_ids = cand.cand_ids;
-  r.cand_scores = cand.cand_scores;
+  r.cand_ids = cand_ids;
+  r.cand_scores = cand_scores;
   return rc;
 }
 
@@ -715,6 +726,20 @@ extern "C" int crag_ivf_search(const void* residuals, int64_t n_rows_padded, int
 }
 
 // ------------------------------------------------------------------ IVF over int8 residuals (ivf_passes with a rescore)
+namespace crag {
+namespace {
+// the int8 residuals and queries of an int8 IVF search: dim8 = dim rounded up to 128, the scan's operand rules, scales
+int check_ivf_i8_codes(const char* who, int dim, const Operand& res, const Operand& q, const float* row_scales,
+                       const float* query_scales) {
+  if (res.width != (dim + 127) / 128 * 128) return fail(CRAG_ERR_INVALID, "%s: dim8 must be dim rounded up to a multiple of 128 (dim=%d dim8=%d)", who, dim, res.width);
+  int rc = check_operand(who, res);
+  if (rc == CRAG_OK) rc = check_operand(who, q);
+  if (rc == CRAG_OK && (!row_scales || !query_scales)) rc = fail(CRAG_ERR_INVALID, "%s: null pointer", who);
+  return rc;
+}
+}  // namespace
+}  // namespace crag
+
 extern "C" size_t crag_ivf_i8_workspace_bytes(int nlist, int64_t total_tiles, int n_cand) {
   if (nlist < 1 || total_tiles < 0 || n_cand < 1 || n_cand > 128) return 0;
   return plan_ivf_i8(nlist, total_tiles, n_cand).total;
@@ -733,14 +758,9 @@ extern "C" int crag_ivf_search_i8(const void* residuals_i8, const float* row_sca
                      {queries_bf16, nq, dim, dim, kBf16, "queries_bf16"}, nullptr, nullptr};
   const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
   const IvfI8Plan plan = plan_ivf_i8(nlist, total_tiles, n_cand, workspace);
-  const int rc = check_rescored_ivf("ivf_i8", lists, n_rows_padded, nq, n_cand, k, out_ids, out_scores, rescore, plan,
-                                    workspace, workspace_bytes, plan.total, [&] {
-    if (dim8 != (dim + 127) / 128 * 128) return fail(CRAG_ERR_INVALID, "ivf_i8: dim8 must be dim rounded up to a multiple of 128 (dim=%d dim8=%d)", dim, dim8);
-    int rc = check_operand("ivf_i8", res);
-    if (rc == CRAG_OK) rc = check_operand("ivf_i8", q);
-    if (rc == CRAG_OK && (!row_scales || !query_scales)) rc = fail(CRAG_ERR_INVALID, "ivf_i8: null pointer");
-    return rc;
-  });
+  const int rc = check_rescored_ivf("ivf_i8", lists, n_rows_padded, nq, n_cand, k, 128, out_ids, out_scores, rescore,
+                                    plan.cand_ids, plan.cand_scores, workspace, workspace_bytes, plan.total,
+                                    [&] { return check_ivf_i8_codes("ivf_i8", dim, res, q, row_scales, query_scales); });
   if (rc != CRAG_OK) return rc;
   return ivf_scan_passes(res, q, I8IvfArgs{{}, {row_scales, query_scales}}, lists, n_cand, k, &rescore, out_ids, out_scores,
                          out_minmax, plan.ivf, static_cast<cudaStream_t>(stream));
@@ -771,6 +791,16 @@ int check_pq_shape(const char* who, int dim, int m) {
   return CRAG_OK;
 }
 
+// the codes and codebooks of a PQ IVF search
+int check_ivf_pq_codes(const char* who, int dim, int m, const void* codes, int64_t code_stride, const float* codebooks) {
+  const int rc = check_pq_shape(who, dim, m);
+  if (rc != CRAG_OK) return rc;
+  if (code_stride < pq_code_stride(m) || code_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "%s: code_stride must be a multiple of 16 and >= %d (code_stride=%lld)", who, pq_code_stride(m), (long long)code_stride);
+  if (!codes || !codebooks) return fail(CRAG_ERR_INVALID, "%s: null codes or codebooks pointer", who);
+  if ((reinterpret_cast<uintptr_t>(codes) | reinterpret_cast<uintptr_t>(codebooks)) & 15) return fail(CRAG_ERR_INVALID, "%s: codes and codebooks must be 16-byte aligned", who);
+  return CRAG_OK;
+}
+
 }  // namespace
 }  // namespace crag
 
@@ -790,15 +820,9 @@ extern "C" int crag_ivf_search_pq(const void* codes, int m, int64_t code_stride,
                      {queries_bf16, nq, dim, dim, kBf16, "queries_bf16"}, nullptr, nullptr};
   const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
   const IvfPqPlan plan = plan_ivf_pq(nlist, total_tiles, n_cand, m, workspace);
-  const int rc = check_rescored_ivf("ivf_pq", lists, n_rows_padded, nq, n_cand, k, out_ids, out_scores, rescore, plan.cand,
-                                    workspace, workspace_bytes, plan.total, [&] {
-    const int rc = check_pq_shape("ivf_pq", dim, m);
-    if (rc != CRAG_OK) return rc;
-    if (code_stride < pq_code_stride(m) || code_stride % 16 != 0) return fail(CRAG_ERR_INVALID, "ivf_pq: code_stride must be a multiple of 16 and >= %d (code_stride=%lld)", pq_code_stride(m), (long long)code_stride);
-    if (!codes || !codebooks) return fail(CRAG_ERR_INVALID, "ivf_pq: null codes or codebooks pointer");
-    if ((reinterpret_cast<uintptr_t>(codes) | reinterpret_cast<uintptr_t>(codebooks)) & 15) return fail(CRAG_ERR_INVALID, "ivf_pq: codes and codebooks must be 16-byte aligned");
-    return CRAG_OK;
-  });
+  const int rc = check_rescored_ivf("ivf_pq", lists, n_rows_padded, nq, n_cand, k, 128, out_ids, out_scores, rescore,
+                                    plan.cand.cand_ids, plan.cand.cand_scores, workspace, workspace_bytes, plan.total,
+                                    [&] { return check_ivf_pq_codes("ivf_pq", dim, m, codes, code_stride, codebooks); });
   if (rc != CRAG_OK) return rc;
   // Stage 1: the queries' tables, then the PQ scan for n_cand candidates, about two CTAs per SM in all; every
   // (slice, query) CTA writes its part, so the merge reads `slices` parts.
@@ -821,6 +845,174 @@ extern "C" int crag_ivf_search_pq(const void* codes, int m, int64_t code_stride,
     });
     if (rc != CRAG_OK) return rc;
     CRAG_CUDA_OK(cudaGetLastError());
+    return CRAG_OK;
+  });
+}
+
+// ------------------------------------------------------------------ wide IVF stage 1: up to 2048 candidates per query
+// Per 32-query pass: the IVF plan, the wide plan (slot layout, ivf_kernels.cuh), a score-all fill of every probed row's
+// S1 into the S1 block (ivf_wide_kernels.cuh), the ragged per-query select (knn_select.cuh), the map of slots to stored
+// positions, then the IVF rescore and the id map.  DESIGN.md section 7.
+namespace crag {
+namespace {
+
+constexpr int kIvfWideMaxCand = kKnnMaxK;
+constexpr int64_t kIvfMaxProbeRows = (int64_t(1) << 31) - kTileRows;
+
+// Workspace of the wide searches: the IVF plan (sized for a 1-key scan, which the wide path never launches: only its
+// list mask, coarse terms and work-list are used), the wide plan, the S1 block [kNQ][round_up(max_probe_rows, 4)],
+// the candidates of one pass, then (PQ, m > 0) the tables of one pass's queries.
+struct IvfWideWs {
+  IvfPlan ivf;
+  IvfWidePlan wide;
+  float* block;
+  int64_t ld;
+  int64_t* cand_ids;
+  float* cand_scores;
+  float* lut;
+  size_t total;
+};
+IvfWideWs plan_ivf_wide(int nlist, int64_t total_tiles, int n_cand, int64_t max_probe_rows, int m, const void* ws = nullptr) {
+  IvfWideWs p;
+  p.ivf = plan_ivf(1, nlist, total_tiles, ws);
+  WsCursor c(ws, p.ivf.total);
+  p.wide.slot_base = c.take<int32_t>(size_t(nlist) * kNQ);
+  p.wide.seg_list = c.take<int32_t>(size_t(kNQ) * kIvfMaxProbe);
+  p.wide.seg_slot = c.take<int32_t>(size_t(kNQ) * kIvfMaxProbe);
+  p.wide.n_seg = c.take<int32_t>(kNQ);
+  p.wide.n_rows = c.take<int32_t>(kNQ);
+  p.ld = (max_probe_rows + 3) & ~int64_t(3);
+  p.block = c.take<float>(size_t(kNQ) * size_t(p.ld));
+  p.cand_ids = c.take<int64_t>(size_t(kNQ) * n_cand);
+  p.cand_scores = c.take<float>(size_t(kNQ) * n_cand);
+  p.lut = c.take<float>(size_t(kNQ) * m * kPqCodewords);
+  p.total = c.bytes;
+  return p;
+}
+
+bool wide_sizes_ok(int nlist, int64_t total_tiles, int n_cand, int64_t max_probe_rows) {
+  return nlist >= 1 && total_tiles >= 0 && n_cand >= 1 && n_cand <= kIvfWideMaxCand && max_probe_rows >= 1 &&
+         max_probe_rows <= kIvfMaxProbeRows;
+}
+
+// The workspace layout of a wide search's arguments.  Sizes out of range are refused by the argument checks before the
+// layout is used, so they carve a minimal one.
+IvfWideWs plan_ivf_wide_args(int nlist, int64_t total_tiles, int n_cand, int64_t max_probe_rows, int m, const void* ws) {
+  if (!wide_sizes_ok(nlist, total_tiles, n_cand, max_probe_rows)) return plan_ivf_wide(1, 0, 1, 1, 0, ws);
+  return plan_ivf_wide(nlist, total_tiles, n_cand, max_probe_rows, m >= 1 && m <= kPqMaxM ? m : 0, ws);
+}
+
+// the wide forms' own rules beside their entry's: max_probe_rows, and nprobe within the wide plan's probe table
+int check_wide_rows(const char* who, int nprobe, int64_t max_probe_rows) {
+  if (max_probe_rows < 1 || max_probe_rows > kIvfMaxProbeRows) return fail(CRAG_ERR_INVALID, "%s: need 1 <= max_probe_rows <= %lld (max_probe_rows=%lld)", who, (long long)kIvfMaxProbeRows, (long long)max_probe_rows);
+  if (nprobe > kIvfMaxProbe) return fail(CRAG_ERR_INVALID, "%s: need nprobe <= %d (nprobe=%d)", who, kIvfMaxProbe, nprobe);
+  return CRAG_OK;
+}
+
+// The passes of a wide search.  `fill(q0, nqc, slices, args, out)` launches the score-all fill of the pass's S1 block
+// over nqc * slices CTAs, about ctas_per_sm per SM: 2 for the PQ fill, as the PQ scan, and 8 for the int8 fill, whose
+// one-warp-per-row CTAs need more warps per SM to keep enough row reads in flight.
+template <class Fill>
+int ivf_wide_passes(int nq, const IvfLists& l, int n_cand, int k, int cap, const IvfRescore& rescore, int64_t* out_ids,
+                    float* out_scores, float* out_minmax, const IvfWideWs& w, cudaStream_t stream, int ctas_per_sm,
+                    Fill fill) {
+  const IvfPlan& ip = w.ivf;
+  const IvfArgs args{ip.work, ip.n_work, ip.list_mask, ip.coarse};
+  const IvfWideBlock out{l.tile_start, w.wide.slot_base, w.block, w.ld, cap};
+  const int grid = ip.scan.grid;
+  return ivf_pass_loop(nq, l, k, out_ids, out_scores, out_minmax, ip, stream,
+                       [&](int q0, int nqc, int64_t* ids, float* scores, float* minmax) {
+    ivf_wide_plan_kernel<<<nqc, kIvfMaxProbe, 0, stream>>>(l.probed_ids + size_t(q0) * l.nprobe, l.nprobe, l.nlist, l.rows,
+                                                           cap, w.wide);
+    CRAG_CUDA_OK(cudaGetLastError());
+    // about ctas_per_sm CTAs per SM in all, at most half of them for one query
+    const int slices = std::min(ctas_per_sm * grid / 2, std::max(1, (ctas_per_sm * grid + nqc - 1) / nqc));
+    int rc = fill(q0, nqc, slices, args, out);
+    if (rc != CRAG_OK) return rc;
+    CRAG_CUDA_OK(cudaGetLastError());
+    ivf_wide_select_kernel<<<nqc, kKnnThreads, 0, stream>>>(w.block, w.ld, w.wide.n_rows, n_cand, w.cand_ids,
+                                                            w.cand_scores, minmax);
+    CRAG_CUDA_OK(cudaGetLastError());
+    ivf_slot_map_kernel<<<(nqc * n_cand + 255) / 256, 256, 0, stream>>>(w.cand_ids, nqc, n_cand, w.wide, l.tile_start);
+    CRAG_CUDA_OK(cudaGetLastError());
+    return launch_ivf_rescore(rescore.rows.ptr, rescore.rows.rows, rescore.rows.width, rescore.rows.stride,
+                              rescore.queries.rows_from(q0, nqc).ptr, nqc, w.cand_ids, n_cand, k, l.tile_start, l.nlist,
+                              ip.coarse, ids, scores, stream);
+  });
+}
+
+}  // namespace
+}  // namespace crag
+
+extern "C" size_t crag_ivf_i8_wide_workspace_bytes(int nlist, int64_t total_tiles, int n_cand, int64_t max_probe_rows) {
+  if (!wide_sizes_ok(nlist, total_tiles, n_cand, max_probe_rows)) return 0;
+  return plan_ivf_wide(nlist, total_tiles, n_cand, max_probe_rows, 0).total;
+}
+
+extern "C" size_t crag_ivf_pq_wide_workspace_bytes(int nlist, int64_t total_tiles, int n_cand, int64_t max_probe_rows,
+                                                   int m) {
+  if (!wide_sizes_ok(nlist, total_tiles, n_cand, max_probe_rows) || m < 1 || m > kPqMaxM) return 0;
+  return plan_ivf_wide(nlist, total_tiles, n_cand, max_probe_rows, m).total;
+}
+
+extern "C" int crag_ivf_search_i8_wide(const void* residuals_i8, const float* row_scales, int dim8, int64_t row_stride_i8,
+                                       const void* residuals_bf16, int dim, int64_t row_stride, int64_t n_rows_padded,
+                                       const int32_t* list_tile_start, const int32_t* list_rows, int nlist,
+                                       int64_t total_tiles, const int64_t* row_ids, const void* queries_i8,
+                                       const float* query_scales, const void* queries_bf16, int nq,
+                                       const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand,
+                                       int k, int64_t max_probe_rows, int64_t* out_ids, float* out_scores,
+                                       float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream) {
+  const char* who = "ivf_i8_wide";
+  const Operand res{residuals_i8, n_rows_padded, dim8, row_stride_i8, kS8, "residuals_i8"}, q{queries_i8, nq, dim8, dim8, kS8, "queries_i8"};
+  IvfRescore rescore{{residuals_bf16, n_rows_padded, dim, row_stride, kBf16, "residuals_bf16"},
+                     {queries_bf16, nq, dim, dim, kBf16, "queries_bf16"}, nullptr, nullptr};
+  const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
+  const IvfWideWs plan = plan_ivf_wide_args(nlist, total_tiles, n_cand, max_probe_rows, 0, workspace);
+  const int rc = check_rescored_ivf(who, lists, n_rows_padded, nq, n_cand, k, kIvfWideMaxCand, out_ids, out_scores, rescore,
+                                    plan.cand_ids, plan.cand_scores, workspace, workspace_bytes, plan.total, [&] {
+    const int rc = check_wide_rows(who, nprobe, max_probe_rows);
+    return rc != CRAG_OK ? rc : check_ivf_i8_codes(who, dim, res, q, row_scales, query_scales);
+  });
+  if (rc != CRAG_OK) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return ivf_wide_passes(nq, lists, n_cand, k, int(max_probe_rows), rescore, out_ids, out_scores, out_minmax, plan, st, 8,
+                         [&](int q0, int nqc, int slices, const IvfArgs& args, const IvfWideBlock& out) {
+    ivf_fill_i8_kernel<<<unsigned(nqc * slices), kIvfFillThreads, 0, st>>>(
+        static_cast<const int8_t*>(residuals_i8), row_stride_i8, dim8, row_scales,
+        static_cast<const int8_t*>(queries_i8) + size_t(q0) * dim8, query_scales + q0, slices, args, out);
+    return CRAG_OK;
+  });
+}
+
+extern "C" int crag_ivf_search_pq_wide(const void* codes, int m, int64_t code_stride, const float* codebooks,
+                                       const void* residuals_bf16, int dim, int64_t row_stride, int64_t n_rows_padded,
+                                       const int32_t* list_tile_start, const int32_t* list_rows, int nlist,
+                                       int64_t total_tiles, const int64_t* row_ids, const void* queries_bf16, int nq,
+                                       const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand,
+                                       int k, int64_t max_probe_rows, int64_t* out_ids, float* out_scores,
+                                       float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream) {
+  const char* who = "ivf_pq_wide";
+  IvfRescore rescore{{residuals_bf16, n_rows_padded, dim, row_stride, kBf16, "residuals_bf16"},
+                     {queries_bf16, nq, dim, dim, kBf16, "queries_bf16"}, nullptr, nullptr};
+  const IvfLists lists{list_tile_start, list_rows, nlist, total_tiles, row_ids, probed_ids, probed_scores, nprobe};
+  const IvfWideWs plan = plan_ivf_wide_args(nlist, total_tiles, n_cand, max_probe_rows, m, workspace);
+  const int rc = check_rescored_ivf(who, lists, n_rows_padded, nq, n_cand, k, kIvfWideMaxCand, out_ids, out_scores, rescore,
+                                    plan.cand_ids, plan.cand_scores, workspace, workspace_bytes, plan.total, [&] {
+    const int rc = check_wide_rows(who, nprobe, max_probe_rows);
+    return rc != CRAG_OK ? rc : check_ivf_pq_codes(who, dim, m, codes, code_stride, codebooks);
+  });
+  if (rc != CRAG_OK) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return ivf_wide_passes(nq, lists, n_cand, k, int(max_probe_rows), rescore, out_ids, out_scores, out_minmax, plan, st, 2,
+                         [&](int q0, int nqc, int slices, const IvfArgs& args, const IvfWideBlock& out) {
+    const void* qp = rescore.queries.rows_from(q0, nqc).ptr;
+    pq_table_kernel<<<unsigned(nqc * m), kPqTableThreads, 0, st>>>(static_cast<const uint16_t*>(qp), dim, codebooks, m, plan.lut);
+    CRAG_CUDA_OK(cudaGetLastError());
+    const int rc = allow_dynamic_smem<ivf_fill_pq_kernel>(size_t(kPqMaxM) * kPqCodewords * 4);
+    if (rc != CRAG_OK) return rc;
+    ivf_fill_pq_kernel<<<unsigned(nqc * slices), kIvfFillThreads, size_t(m) * kPqCodewords * 4, st>>>(
+        static_cast<const uint8_t*>(codes), code_stride, m, plan.lut, slices, args, out);
     return CRAG_OK;
   });
 }

@@ -26,7 +26,7 @@ import numpy as np
 import torch
 
 from . import _native
-from .index import DenseIndex, MAX_K
+from .index import DenseIndex, KNN_MAX_K, MAX_K
 from .quantized import _dim8, check_place, place_rows, quantize_rows, rescored_candidates
 
 TILE_ROWS = 128
@@ -228,6 +228,41 @@ class _RescoredIVF(_IVFSearch):
         self.total_tiles = ivf.total_tiles
         self._rows = residuals_bf16     # bf16 [total_tiles * 128, dim], on the device or in page-locked host memory
         self._lib = _native.load()
+        # list sizes, largest first, for probe_rows_bound (snapshots are built after place_rows has synchronised)
+        self._rows_desc = np.sort(ivf.list_rows.cpu().numpy().astype(np.int64))[::-1]
+
+    def probe_rows_bound(self, nprobe: int) -> int:
+        """The most real rows a query probing `nprobe` distinct lists can see: the rows of the nprobe largest lists."""
+        return int(self._rows_desc[:nprobe].sum())
+
+    def _wide_fine(self, nprobe: int, candidates: int, k: int, max_probe_rows: int):
+        """(workspace bytes, fine pass) of the subclass's wide C entry, as _IVFSearch._search takes them."""
+        raise NotImplementedError
+
+    def search_device_wide(self, queries_bf16: torch.Tensor, nprobe: int, k: int, candidates: int,
+                           stream: Optional[torch.cuda.Stream] = None,
+                           probed: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
+        """search_device for up to 2048 candidates (1 <= k <= candidates <= 2048), with search_device's tuple.  At most
+        128 it is search_device; above, stage 1 scores every probed row into a block of probe_rows_bound(nprobe)
+        slots per query and keeps the exact top `candidates` by stage-1 score (crag_ivf_search_i8_wide /
+        crag_ivf_search_pq_wide), and the rescore sorts them all."""
+        if not 1 <= k <= candidates <= KNN_MAX_K:
+            raise ValueError(f"need 1 <= k <= candidates <= {KNN_MAX_K} (k={k}, candidates={candidates})")
+        if candidates <= MAX_K:
+            return self.search_device(queries_bf16, nprobe, k, candidates, stream, probed)
+        ws_bytes, fine = self._wide_fine(nprobe, candidates, k, max(1, self.probe_rows_bound(nprobe)))
+        return self._search(queries_bf16, nprobe, k, stream, probed, ws_bytes, fine)
+
+    def search_wide(self, queries, nprobe: int, k: int, candidates: int, *args, **kw) -> Tuple[np.ndarray, np.ndarray]:
+        """search_device_wide's host twin, as search is search_device's."""
+        if not 1 <= k <= candidates <= KNN_MAX_K:
+            raise ValueError(f"need 1 <= k <= candidates <= {KNN_MAX_K} (k={k}, candidates={candidates})")
+        q = torch.as_tensor(queries)
+        if q.dim() == 1:
+            q = q[None, :]
+        q = q.to(self.device, non_blocking=True).to(torch.bfloat16)
+        ids, scores, _, _ = self.search_device_wide(q, nprobe, k, candidates, *args, **kw)
+        return ids.cpu().numpy(), scores.cpu().numpy()
 
     @property
     def residuals_on_device(self) -> bool:
@@ -291,6 +326,19 @@ class QuantizedIVF(_RescoredIVF):
                 "crag_ivf_search_i8")
         return self._search(queries_bf16, nprobe, k, stream, probed,
                             self._lib.crag_ivf_i8_workspace_bytes(self.nlist, self.total_tiles, candidates), fine)
+
+    def _wide_fine(self, nprobe: int, candidates: int, k: int, max_probe_rows: int):
+        def fine(q, p_ids, p_scores, ids, scores, minmax, ws, st):
+            q8, qs = quantize_rows(q, self.dim8, st)
+            _native.check(self._lib.crag_ivf_search_i8_wide(
+                self._i8.data_ptr(), self._scales.data_ptr(), self.dim8, self._i8.stride(0),
+                self._rows.data_ptr(), self.dim, self._rows.stride(0), self._rows.shape[0],
+                self.list_tile_start.data_ptr(), self.list_rows.data_ptr(), self.nlist, self.total_tiles,
+                self.row_ids.data_ptr(), q8.data_ptr(), qs.data_ptr(), q.data_ptr(), q.shape[0],
+                p_ids.data_ptr(), p_scores.data_ptr(), nprobe, candidates, k, max_probe_rows,
+                ids.data_ptr(), scores.data_ptr(), minmax.data_ptr(), ws.data_ptr(), ws.numel(), st.cuda_stream),
+                "crag_ivf_search_i8_wide")
+        return self._lib.crag_ivf_i8_wide_workspace_bytes(self.nlist, self.total_tiles, candidates, max_probe_rows), fine
 
 
 class ShardedIVF:

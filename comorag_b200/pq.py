@@ -137,3 +137,15 @@ class PQIVF(_RescoredIVF):
                 st.cuda_stream), "crag_ivf_search_pq")
         return self._search(queries_bf16, nprobe, k, stream, probed,
                             self._lib.crag_ivf_pq_workspace_bytes(self.nlist, self.total_tiles, candidates, self.m), fine)
+
+    def _wide_fine(self, nprobe: int, candidates: int, k: int, max_probe_rows: int):
+        def fine(q, p_ids, p_scores, ids, scores, minmax, ws, st):
+            _native.check(self._lib.crag_ivf_search_pq_wide(
+                self.codes.data_ptr(), self.m, self.codes.stride(0), self.codebooks.data_ptr(),
+                self._rows.data_ptr(), self.dim, self._rows.stride(0), self._rows.shape[0],
+                self.list_tile_start.data_ptr(), self.list_rows.data_ptr(), self.nlist, self.total_tiles,
+                self.row_ids.data_ptr(), q.data_ptr(), q.shape[0], p_ids.data_ptr(), p_scores.data_ptr(), nprobe,
+                candidates, k, max_probe_rows, ids.data_ptr(), scores.data_ptr(), minmax.data_ptr(), ws.data_ptr(),
+                ws.numel(), st.cuda_stream), "crag_ivf_search_pq_wide")
+        return (self._lib.crag_ivf_pq_wide_workspace_bytes(self.nlist, self.total_tiles, candidates, max_probe_rows,
+                                                           self.m), fine)

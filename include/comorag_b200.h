@@ -416,6 +416,36 @@ CRAG_API int crag_ivf_search_pq(const void* codes, int m, int64_t code_stride, c
                                 const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand, int k,
                                 int64_t* out_ids, float* out_scores, float* out_minmax, void* workspace,
                                 size_t workspace_bytes, crag_stream_t stream);
+/* Wide forms of crag_ivf_search_i8 and crag_ivf_search_pq: up to 2048 candidates per query.  Same arguments plus
+ * max_probe_rows, and 1 <= k <= n_cand <= 2048, nprobe <= 128, 1 <= max_probe_rows < 2^31 - 128.  Stage 1 writes S1
+ * (bit for bit the narrow entry's) of every probed row of a 32-query pass into a fp32 block [32, round_up(max_probe_rows,
+ * 4)] of the workspace, in slot order: the query's distinct valid probes in ascending list id, rows in stored order
+ * inside a list, so slot order is stored-position order.  A query with more probed rows than max_probe_rows keeps its
+ * first max_probe_rows slots; with max_probe_rows >= the rows of the nprobe largest lists none is dropped.  Then one
+ * CTA per query radix-selects the exact top n_cand by (S1 desc, position asc) -- the narrow entry's candidate set up to
+ * 128, and the smaller set a prefix of the larger for any two counts -- and the rescore, id map and outputs are the
+ * narrow entry's.  out_minmax is (min, max) of S1 over the scored rows.
+ * workspace >= crag_ivf_i8_wide_workspace_bytes(nlist, total_tiles, n_cand, max_probe_rows) or
+ * crag_ivf_pq_wide_workspace_bytes(nlist, total_tiles, n_cand, max_probe_rows, m), 256-byte aligned (0 for bad
+ * arguments). */
+CRAG_API size_t crag_ivf_i8_wide_workspace_bytes(int nlist, int64_t total_tiles, int n_cand, int64_t max_probe_rows);
+CRAG_API int crag_ivf_search_i8_wide(const void* residuals_i8, const float* row_scales, int dim8, int64_t row_stride_i8,
+                                     const void* residuals_bf16, int dim, int64_t row_stride, int64_t n_rows_padded,
+                                     const int32_t* list_tile_start, const int32_t* list_rows, int nlist,
+                                     int64_t total_tiles, const int64_t* row_ids, const void* queries_i8,
+                                     const float* query_scales, const void* queries_bf16, int nq,
+                                     const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand,
+                                     int k, int64_t max_probe_rows, int64_t* out_ids, float* out_scores,
+                                     float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream);
+CRAG_API size_t crag_ivf_pq_wide_workspace_bytes(int nlist, int64_t total_tiles, int n_cand, int64_t max_probe_rows,
+                                                 int m);
+CRAG_API int crag_ivf_search_pq_wide(const void* codes, int m, int64_t code_stride, const float* codebooks,
+                                     const void* residuals_bf16, int dim, int64_t row_stride, int64_t n_rows_padded,
+                                     const int32_t* list_tile_start, const int32_t* list_rows, int nlist,
+                                     int64_t total_tiles, const int64_t* row_ids, const void* queries_bf16, int nq,
+                                     const int64_t* probed_ids, const float* probed_scores, int nprobe, int n_cand,
+                                     int k, int64_t max_probe_rows, int64_t* out_ids, float* out_scores,
+                                     float* out_minmax, void* workspace, size_t workspace_bytes, crag_stream_t stream);
 /* Product-quantizer encode (also the assignment step of codebook training): for every row r and subspace j,
  * codes[r * code_stride + j] = argmin_c sum_t (r_{j,t} - C_j[c][t])^2 over the bf16 row read as fp32 (fp32, t order,
  * no FMA, ties to the smaller c).  rows bf16 [n_rows, row_stride] (device or page-locked host memory); codebooks device
